@@ -19,12 +19,16 @@ rank keeps 64 images).  Prints ONE JSON line on rank 0.
              bounded sample
   gpu_library_baseline  (N=1) the reference's own eager CUDA forward -- the module's nn.Conv2d / BatchNorm2d / ReLU6 /
              F.interpolate children run by PyTorch + cuDNN (cudnn.benchmark=True), fp16 and fp32, NCHW and channels_last --
-             on the same B200: the existing-Blackwell-library bar (SURVEY.md 8d).  Outside the product's timed region.
+             on the same GPU: the existing-library bar (SURVEY.md 8d).  Outside the product's timed region.
   eval       BASELINE config 4's shape: bf16, 64 images per rank, per-image metrics on device, ONE all-reduce(SUM) of
              11 doubles (NCCL under torchrun); prints delta1 / RMSE next to the oracle's, the all-reduce time and whether
              the N-rank sums equal the sums of a single rank that ran every image (bit for bit, fp64)
-  --impl reference : times ONLY that CPU implementation (the reference is pure Python on PyTorch;
-             /root/reference does not exist on the GPU box, so the oracle port stands in).
+  --impl reference : times ONLY that CPU implementation (the reference is pure Python on PyTorch and
+             not part of this repository, so the oracle port stands in).
+  --dump-outputs DIR : after the timed steps, writes the depth maps the timed path produced in its last step as
+             DIR/depth.npy (float32, [batch, 1, H, W]; above 64 MB a fixed seeded sample of whole images, listed in
+             DIR/depth_images.npy).  Inputs and weights are seeded, so two builds run with the same arguments can be
+             compared output for output.
 """
 import argparse
 import json
@@ -62,22 +66,38 @@ def parse():
     ap.add_argument('--no-lib-baseline', action='store_true', help='skip the cuDNN-eager leg')
     ap.add_argument('--no-eval', action='store_true', help='skip the bf16 sharded-evaluation leg (config 4)')
     ap.add_argument('--e2e-steps', type=int, default=200)
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the timed path computed in its last step as DIR/<name>.npy (float32)')
     ap.add_argument('--lanes', type=int, default=3, help='batches in flight: independent plan copies on their own streams '
                                                          '(fastdepth_b200.engine.ForwardLanes); 1 = strict single stream')
     return ap.parse_args()
 
 
 def peaks():
-    """(HBM GB/s, sustained dense 16-bit TFLOP/s, SM MHz, source)"""
-    p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return (float(d['hbm_gbs']), float(d.get('bf16_tflops_sustained', 1467.7)), float(d.get('sm_max_mhz', 1965.0)),
-                'measured (MEASURED_PEAKS.json hbm_gbs burst copy; bf16_tflops_sustained)')
-    return 6650.0, 1400.0, 1965.0, 'fallback (B200_PROFILING.md)'
+    """(HBM GB/s, dense 16-bit TFLOP/s, SM MHz, source): NVIDIA's H100 SXM data sheet (700 W card); a card run at a lower
+    power limit reaches less, so fractions of these are lower bounds on the share of the card's real capability."""
+    return 3350.0, 989.0, 1980.0, 'H100 SXM data sheet (700 W)'
 
 
-NOMINAL_HBM_GBS = 8000.0        # the figure north_star quotes
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, y):
+    """DIR/depth.npy: the depth maps [N, 1, H, W] as float32.  Above DUMP_CAP_BYTES only a fixed, seeded sample of whole
+    images is written, and DIR/depth_images.npy (float64) lists which images of the batch they are."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize(y.device)
+    n = y.shape[0]
+    per_image = y[0].numel() * 4
+    if n * per_image > DUMP_CAP_BYTES:
+        keep = np.sort(np.random.default_rng(0).choice(n, max(1, DUMP_CAP_BYTES // per_image), replace=False))
+        np.save(os.path.join(out_dir, 'depth_images.npy'), keep.astype(np.float64))
+        y = y[torch.from_numpy(keep).to(y.device)]
+    np.save(os.path.join(out_dir, 'depth.npy'), y.float().cpu().numpy())
+
+
+NOMINAL_HBM_GBS = 3350.0        # H100 SXM data-sheet HBM3 bandwidth
 
 
 def eager_reference_forward(model, x):
@@ -337,7 +357,7 @@ def run_reference(args, rank):
                                (args.widths, h, w), 'batch_per_step': batch, 'global_batch': batch},
         'cpu_baseline': {'value': rate, 'unit': UNIT, 'cores': cores, 'kind': 'port',
                          'sample': '%d steps of batch %d (fp32, torch CPU, NCHW) -- the reference is pure Python on '
-                                   'PyTorch and /root/reference is absent on the GPU box, so the oracle port runs; %s' % (steps, batch, thread_note)},
+                                   'PyTorch and not part of this repository, so the oracle port runs; %s' % (steps, batch, thread_note)},
         'e2e': {'value': rate, 'unit': UNIT, 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
         'gpu_launches': 0,
     }
@@ -350,6 +370,8 @@ def main():
     local_rank = int(os.environ.get('LOCAL_RANK', 0))
     world = int(os.environ.get('WORLD_SIZE', 1))
     if args.impl == 'reference':
+        if args.dump_outputs:
+            raise SystemExit('--dump-outputs dumps the GPU path; the reference arm has nothing to compare with it')
         run_reference(args, rank)
         return
 
@@ -381,7 +403,7 @@ def main():
     lanes = ForwardLanes(model, lanes=R, options=opts)
 
     # 4 rotating input batches (different images per rank); a step moves >1 GB through HBM, far more
-    # than the 126 MB L2, so nothing of the previous step's input survives in cache.
+    # than the 50 MB L2, so nothing of the previous step's input survives in cache.
     n_rot = 4
     xs = [synthetic.synthetic_input(n, h, w, seed=100 * rank + i).to(dev).to(dtype) for i in range(n_rot)]
     y = torch.empty((n, 1, h, w), dtype=dtype, device=dev)
@@ -429,6 +451,8 @@ def main():
                          args.steps, max(3, args.warmup) * R, fan=lane_streams)
     else:
         ms_total = ms_single
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, lane_y[(args.steps - 1) % R] if R > 1 else y)   # the buffer the last timed step wrote
     # ---- e2e: pinned host buffers through the C-ABI pipeline (fd_pipeline_submit / fd_pipeline_wait): every step
     # uploads its batch from pinned host memory and downloads its depth maps; up to 3 batches are in flight so
     # the PCIe copies overlap the forward of the neighbouring steps.  Timed on the host clock between device-wide
@@ -492,21 +516,12 @@ def main():
         s['tflops'] = 2 * s['macs'] / (s['ms'] * 1e-3) / 1e12 if s['ms'] > 0 else 0.0
         s['dense_tflops'] = 2 * s['dense_macs'] / (s['ms'] * 1e-3) / 1e12 if s['ms'] > 0 else 0.0
         # the three floors of a fused stage: HBM (algorithmic bytes), the SIMT FMA pipe for the depthwise taps (128 FMA lanes
-        # per SM and clock, north_star keeps them off the tensor cores) and the tensor pipe for the dense contraction
+        # per SM and clock; the depthwise taps do not run on the tensor cores) and the tensor pipe for the dense contraction
         s['hbm_floor_us'] = s['alg_bytes'] / (hbm_peak * 1e9) * 1e6
         s['fma_floor_us'] = s['dw_macs'] / (n_sms * 128.0 * sm_mhz * 1e6) * 1e6
         s['tensor_floor_us'] = 2 * s['dense_macs'] / (tensor_peak * 1e12) * 1e6
         s['floor_us'] = max(s['hbm_floor_us'], s['fma_floor_us'], s['tensor_floor_us'])
     top = max(steps, key=lambda s: s['ms'])
-    # DRAM traffic of that kernel from the committed `ncu --set full` capture of the same configuration (if any)
-    traffic = None
-    tpath = os.path.join(ROOT, 'profiles', 'r02_final_traffic.json')
-    if not os.path.exists(tpath):
-        tpath = os.path.join(ROOT, 'profiles', 'r01_final_traffic.json')
-    if os.path.exists(tpath) and args.widths == 'stock' and args.dtype == 'fp16' and n == 64 and (h, w) == (224, 224) and args.path == 1:
-        tj = json.load(open(tpath))['stages'].get(top['stage_name'])
-        if tj:
-            traffic = (tj['dram_read_mb'] + tj['dram_write_mb']) * 1e6
     sum_ms = sum(s['ms'] for s in steps)
     alg_total = sum(s['alg_bytes'] for s in steps)
 
@@ -546,7 +561,7 @@ def main():
                    'in_flight': R, 'in_flight_note': '%d independent forwards in flight (plan copies with their own activation buffers on their '
                                                      'own streams, fastdepth_b200.engine.ForwardLanes): every step is a '
                                                      'complete forward of its own batch; the strict single-stream replay is `single_stream`' % R,
-                   'l2': '4 rotating input batches; one step streams %.2f GB through HBM (>> 126 MB L2)' % (alg_total / 1e9),
+                   'l2': '4 rotating input batches; one step streams %.2f GB through HBM (>> 50 MB L2)' % (alg_total / 1e9),
                    'weights': 'random-init (synthetic recipe seed 1)'},
         'e2e': {'value': e2e_value, 'unit': UNIT, 'h2d_bytes_per_step': xh[0].numel() * xh[0].element_size(),
                 'd2h_bytes_per_step': yh[0].numel() * yh[0].element_size(), 'ms_per_step': ms_e2e / e2e_steps,
@@ -558,14 +573,12 @@ def main():
         'gpu_launches': plan.launches_per_forward() * args.steps,
         'launches_per_step': plan.launches_per_forward(),
         'clocks': clocks,
-        # the dominant kernel's own roofline: a merged multi-layer stage (the conv7..11 chain keeps its intermediates in shared
-        # memory) sits far past the ridge -- its dense contraction, not its 28 MB of external bytes, is what bounds it
+        # the dominant kernel's own roofline, against whichever of its HBM and tensor floors is higher
         'roofline': {**({'bound': 'tensor', 'achieved': top['dense_tflops'], 'peak': tensor_peak, 'unit': 'TFLOP/s',
                          'frac': top['dense_tflops'] / tensor_peak, 'hbm_gbs': top['gbs'], 'hbm_frac': top['frac']}
                         if top['tensor_floor_us'] > top['hbm_floor_us'] else
                         {'bound': 'hbm', 'achieved': top['gbs'], 'peak': hbm_peak, 'unit': 'GB/s', 'frac': top['frac']}),
-                     'frac_nominal_8tbs': top['gbs'] / NOMINAL_HBM_GBS,
-                     'traffic': traffic, 'traffic_source': os.path.basename(tpath) if traffic else None,
+                     'frac_nominal_hbm': top['gbs'] / NOMINAL_HBM_GBS,
                      'kernel': top['kernel'], 'stage': top['stage_name'], 'peak_source': peak_src,
                      'kernel_ms': top['ms'], 'share_of_step': top['ms'] / sum_ms,
                      'alg_bytes': top['alg_bytes'],
@@ -577,12 +590,12 @@ def main():
                      'frac_of_binding_floor': top['floor_us'] / (top['ms'] * 1e3),
                      'whole_step': {'alg_bytes': alg_total, 'gbs_at_value': alg_total / (ms_total / args.steps * 1e-3) / 1e9,
                                     'frac_at_value': alg_total / (ms_total / args.steps * 1e-3) / 1e9 / hbm_peak,
-                                    'frac_nominal_8tbs': alg_total / (ms_total / args.steps * 1e-3) / 1e9 / NOMINAL_HBM_GBS,
+                                    'frac_nominal_hbm': alg_total / (ms_total / args.steps * 1e-3) / 1e9 / NOMINAL_HBM_GBS,
                                     'sum_of_isolated_kernel_ms': sum_ms,
                                     'sum_of_binding_floors_us': sum(s['floor_us'] for s in steps)}},
         'stages': [{'stage': s['stage_name'], 'kernel': s['kernel'], 'ms': round(s['ms'], 5),
                     'alg_mb': round(s['alg_bytes'] / 1e6, 3), 'gbs': round(s['gbs'], 1), 'frac': round(s['frac'], 4),
-                    'frac_8tbs': round(s['gbs'] / NOMINAL_HBM_GBS, 4), 'tflops': round(s['tflops'], 2),
+                    'frac_nominal_hbm': round(s['gbs'] / NOMINAL_HBM_GBS, 4), 'tflops': round(s['tflops'], 2),
                     'hbm_floor_us': round(s['hbm_floor_us'], 2), 'fma_floor_us': round(s['fma_floor_us'], 2),
                     'tensor_floor_us': round(s['tensor_floor_us'], 2),
                     'frac_of_floor': round(s['floor_us'] / (s['ms'] * 1e3), 4) if s['ms'] > 0 else 0.0} for s in steps],

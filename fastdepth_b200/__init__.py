@@ -1,8 +1,8 @@
-"""fastdepth_b200 -- B200-native FastDepth forward path (MobileNetSkipAdd.forward).
+"""fastdepth_b200 -- H100-native FastDepth forward path (MobileNetSkipAdd.forward).
 
 Python host side of the C-ABI in include/fastdepth_b200.h:
 
-  build     in-tree nvcc build of libfastdepth_b200.so (sm_100a)
+  build     in-tree nvcc build of libfastdepth_b200.so (sm_90a)
   _lib      ctypes binding (fails loudly if the library is missing; no fallback)
   plan      BN folding + stage description + Plan wrapper around fd_plan
   engine    lazy per-shape plan cache behind models.MobileNetSkipAdd.forward

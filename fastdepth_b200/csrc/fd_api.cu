@@ -31,7 +31,7 @@ int launch_head(int dtype, const void* in, void* out, const float* w, float scal
 int launch_metrics(int dtype, const void* pred, const float* target, int n, int hw, double* sums, cudaStream_t st);
 int launch_nyu_val_gather(int dtype, const uint8_t* rgb, const float* depth, const int* rows, const int* cols, int n, int h_in,
                           int w_in, int oh, int ow, void* x, float* t, cudaStream_t st);
-// fused tcgen05 block kernel
+// fused wgmma block kernel
 struct BlockTcPlan;   // opaque per-stage state (tensor maps, tile config)
 bool block_tc_supported(int dtype, const StageGeom& g, bool head_fused);
 int block_tc_prepare(int dtype, const BlockArgs& a, const float* head_w, float head_scale, float head_bias, int head_act,
@@ -40,7 +40,7 @@ int block_tc_launch(BlockTcPlan* p, cudaStream_t st, void* head_out);
 void block_tc_destroy(BlockTcPlan* p);
 const char* block_tc_name(BlockTcPlan* p);
 int block_tc_trace(BlockTcPlan* bp, cudaStream_t st, void* head_out, unsigned long long* out_host, int* rows, int* cols);
-// fused multi-layer chain kernel (fd_chain_tc.cu): a run of 3x3 stride-1 blocks on a small map in one 2-CTA-cluster kernel
+// fused multi-layer chain kernel (fd_chain_tc.cu): a run of 3x3 stride-1 blocks on a small map in one kernel on 2-CTA clusters
 struct ChainTcPlan;
 bool chain_tc_supported(int dtype, const StageGeom* g, int n_layers);
 int chain_tc_prepare(int dtype, const BlockArgs* layers, int n_layers, const TcLaunchOpts& opts, ChainTcPlan** out);
@@ -99,7 +99,7 @@ struct Step {
 using namespace fd;
 
 struct fd_plan {
-    int n = 0, h = 0, w = 0, dtype = 0, device = 0, n_sms = 148;
+    int n = 0, h = 0, w = 0, dtype = 0, device = 0, n_sms = 132;
     std::vector<Stage> stages;
     std::vector<Step> steps;
     bool steps_valid = false;
@@ -388,7 +388,7 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages, int n, int h, int 
     if (device < 0 || device >= ndev) return fail(FD_ERR_INVALID, "bad device index");
     cudaDeviceProp prop{};
     FD_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail(FD_ERR_UNSUPPORTED, "fastdepth_b200 is built for sm_100a (B200) only");
+    if (prop.major != 9 || prop.minor != 0) return fail(FD_ERR_UNSUPPORTED, "fastdepth_b200 is built for sm_90a (H100) only");
     DeviceGuard guard(device);
     if (!guard.ok) return fail(FD_ERR_CUDA, "cudaSetDevice failed");
 
@@ -771,7 +771,7 @@ int fd_plan_time_steps(fd_plan* p, const void* x_dev, void* y_dev, void* stream,
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (flush_l2 && !p->l2_flush) {
-        p->l2_flush_bytes = size_t(256) << 20;               // > 126 MB L2
+        p->l2_flush_bytes = size_t(256) << 20;               // > the 50 MB L2
         FD_CUDA_OK(cudaMalloc(&p->l2_flush, p->l2_flush_bytes));
     }
     rc = run_steps(p, x_dev, y_dev, st);                      // make every intermediate valid
@@ -814,13 +814,9 @@ int fd_plan_trace_stage(fd_plan* p, int stage, void* y_dev, void* stream, unsign
 int fd_debug_block_plan(int ksize, int stride, int h_out, int w_out, int n, int c_in, int c_out, int head, int* out, int cap) {
     if (!out || cap < 16) return fail(FD_ERR_INVALID, "need an int[16] output");
     const BlockPlanOut q = block_tc_debug_plan(ksize, stride, h_out, w_out, n, c_in, c_out, head);
-    const int v[16] = {q.ok, q.splits, q.n_cta, q.items, q.kblocks, q.s_in, q.s_a, q.s_b, q.bn, q.nb, q.b_resident, q.epi_groups,
-                       q.n_stg, q.smem_bytes, q.tmem_cols, q.in_stage_stride};
+    const int v[16] = {q.ok, q.splits, q.n_cta, q.items, q.kblocks, q.s_in, q.s_a, q.s_b, q.bn, q.nb, q.b_resident, q.n_stg,
+                       q.smem_bytes, q.in_stage_stride, q.cs, q.dw_teams};
     for (int i = 0; i < 16; ++i) out[i] = v[i];
-    if (cap >= 18) { out[16] = q.nacc; out[17] = q.epi_colsplit; }
-    if (cap >= 19) out[18] = q.epi_wide;
-    if (cap >= 20) out[19] = q.cs;
-    if (cap >= 21) out[20] = q.dw_teams;
     return FD_OK;
 }
 

@@ -9,10 +9,12 @@ constexpr int kPlanAStage = 128 * 128;       // one A operand stage: 128 rows x 
 constexpr int kPlanStg = 16384;              // one epilogue staging tile: 128 px x 64 ch x 2 B
 constexpr int kPlanMaxIn = 6, kPlanMaxA = 4, kPlanMaxB = 16;
 constexpr int kPlanMaxACluster = 6;          // cluster mode: the A ring is filled by several CTAs at once and wants >= cluster size stages
+// An item's accumulator lives in the registers of the two consumer warpgroups (64 pixel rows each): n_cta / 2 fp32 registers per
+// thread, so 128 output channels per item is the most the register file leaves room for next to the other roles.
+constexpr int kPlanMaxNcta = 128;
 #ifndef FD_PLAN_SMALL_SMEM
 // everything that needs 1 KB alignment sits in front of the 128-byte-granular input stages (see the kernel's carve-up): ONE alignment
-// slack, and the budget is the whole 227 KB minus a small margin (round 1: 224 KB and two slacks -- conv2 missed its second staging
-// tile by 8 bytes)
+// slack, and the budget is the whole 227 KB an H100 block may opt into, minus a small margin
 constexpr int kPlanSmemBudget = 227 * 1024 - 128;
 constexpr int kPlanAlignSlack = 1024;
 #else
@@ -26,9 +28,7 @@ struct BlockPlanIn {
     int head;                    // decode_conv6 folded into the epilogue
     int barrier_bytes;           // sizeof(TcBarriers)
     int max_n_cta;               // 0 = no limit; experiments: cap the output channels per item (FD_TC_MAX_NCTA)
-    int no_wide;                 // experiments: 1 = a single epilogue group stays four warps (FD_TC_NO_WIDE)
-    int no_colsplit;             // experiments: 1 = epilogue groups take alternate items even when they could share (FD_TC_NO_COLSPLIT)
-    int n_sms;                   // SMs of the device (one CTA each); 0 = 148 (B200)
+    int n_sms;                   // SMs of the device (one CTA each); 0 = 132 (H100 SXM)
     int even_rings;              // 1: input and A rings get an even number of stages (two depthwise teams on alternate steps); 0 / 2: no constraint
     int cluster_multiwave;       // bring-up only (FD_TC_CLUSTER_MULTIWAVE=1): admit tile-sharing clusters on multi-wave launches
     int cluster;                 // 0 = the cost model may choose cluster mode, 1 = never, 2 / 4 = force that cluster size when the
@@ -36,13 +36,10 @@ struct BlockPlanIn {
 };
 struct BlockPlanOut {
     int ok;
-    int kblocks, cin_pad, splits, n_cta, cpad_all, items, tmem_cols;
+    int kblocks, cin_pad, splits, n_cta, cpad_all, items;
     int in_stage_bytes, dwp_bytes, in_stage_stride;
     int s_in, s_a, s_b, bn, nb, b_resident, b_stage_bytes;
-    int epi_groups, n_stg;       // n_stg = staging tiles in total (epi_groups x 1 or 2)
-    int nacc;                    // TMEM accumulators: 2 of n_cta <= 256 columns, or 1 of up to 512
-    int epi_colsplit;            // 1: both epilogue groups drain every item, alternating 64-column blocks
-    int epi_wide;                // 1: one staging tile, all eight epilogue warps on it (32 columns per warp)
+    int n_stg;                   // epilogue staging tiles: 2 (one tile's TMA store overlaps filling the other), 1, or 0 (folded head)
     int dw_teams;                // 2: two depthwise teams of four warps on alternate K-block steps (needs even s_in and s_a), else 1
     int cs;                      // cluster size: 1, or 2 / 4 CTAs that share one tile -- CTA r computes the depthwise half of the
                                  // K-blocks kb % cs == r, broadcasts its operand tiles to the others through DSMEM and runs the MMAs
@@ -50,28 +47,23 @@ struct BlockPlanOut {
     int smem_bytes;
 };
 
-// Shared-memory search for one choice of (splits, n_cta): ring depths / weight sub-block width / epilogue organisation,
-// scored by what matters for the block at hand (stride-2 blocks stage 72 KB of input per K-block and leave little room;
-// single-K-block blocks want a deep A ring to hide the serial latency of the MMA issue thread).
-inline bool plan_block_smem(const BlockPlanIn& q, BlockPlanOut& p, bool allow_narrow) {
+// Shared-memory search for one choice of (splits, n_cta): ring depths / weight stage width / staging tiles, scored by what
+// matters for the block at hand (stride-2 blocks stage 72 KB of input per K-block and leave little room; single-K-block
+// blocks want a deep A ring so that the depthwise warps never wait for the consumers).
+inline bool plan_block_smem(const BlockPlanIn& q, BlockPlanOut& p) {
     const int splits = p.splits;
-    const int sms = q.n_sms > 0 ? q.n_sms : 148;
+    const int sms = q.n_sms > 0 ? q.n_sms : 132;
     const int fixed = q.barrier_bytes + kPlanAlignSlack + (q.head ? 3 : 2) * p.cpad_all * 4;
     const int total = kPlanSmemBudget - fixed;
     long best = -(1L << 60);
     bool found = false;
-    const int bn_top = p.n_cta < 256 ? p.n_cta : 256;
+    const int bn_top = (p.n_cta + 63) / 64 * 64;                 // whole 64-column wgmma blocks (rows past c_out load as zeros)
     const int per_cta_kb = p.cs > 1 ? (p.kblocks + p.cs - 1) / p.cs : p.kblocks;      // K-blocks whose input tile THIS CTA loads
     for (int s_a = p.cs > 1 ? kPlanMaxACluster : kPlanMaxA; s_a >= 2; --s_a)
-        for (int eg = q.head ? 1 : 3; eg >= 0; --eg) {
+        for (int n_stg = q.head ? 0 : 2; n_stg >= (q.head ? 0 : 1); --n_stg) {
             if (q.even_rings == 1 && p.cs == 1 && (s_a & 1)) continue;
-            // epilogue organisation: 3 = two groups x two tiles, 2 = two groups x one tile, 1 = one group x two, 0 = one x one
-            const int groups = q.head ? 2 : (eg >= 2 ? 2 : 1);
-            const int n_stg = q.head ? 0 : groups * ((eg & 1) ? 2 : 1);
-            if (q.head && eg != 1) continue;
-            if (p.nacc == 1 && groups != 2) continue;      // a single 512-column accumulator is drained by both groups together
             const int avail = total - s_a * kPlanAStage - n_stg * kPlanStg;
-            for (int bn = bn_top;; bn = (bn / 2 + 15) / 16 * 16) {
+            for (int bn = bn_top; bn >= 64; bn -= 64) {
                 const int nb = (p.n_cta + bn - 1) / bn;
                 const int w_all = p.kblocks * nb * bn * 128;
                 const bool can_res = splits == 1 && bn == bn_top && p.kblocks * nb <= kPlanMaxB && w_all <= 64 * 1024;
@@ -86,41 +78,25 @@ inline bool plan_block_smem(const BlockPlanIn& q, BlockPlanOut& p, bool allow_na
                         if (q.even_rings && p.cs == 1 && s_in > 4) s_in &= ~1;        // beyond four stages depth buys nothing: keep the ring even
                         if (s_in < 2 && !(s_in == 1 && p.kblocks == 1 && p.items <= sms)) continue;
                         if (p.cs > 1 && s_in > per_cta_kb + 1) s_in = per_cta_kb + 1 < 2 ? 2 : per_cta_kb + 1;
-                        const int bn_eff = bn < 128 ? bn : 128;
-                        // weight ring depth in K-blocks: below 2 the MMA of K-block k+1 waits for a weight load that could
-                        // only start when the MMA of K-block k had finished (measured: conv7 lost a third of its time there)
+                        // weight ring depth in K-blocks: below 2 the MMA of K-block k+1 waits for a weight load that can only
+                        // start when the MMA of K-block k has finished
                         const int b_ahead2 = res ? 4 : (2 * s_b / nb > 4 ? 4 : 2 * s_b / nb);      // in half K-blocks, capped at 2 K-blocks
-                        long score = (long)bn_eff * 100 + (bn >= 256 ? 500 : 0) + (s_in > 4 ? 4 : s_in) * 2500 +
-                                     s_a * (p.kblocks <= 2 ? 1500 : 400) + groups * 2500 + n_stg * 300 + (res ? 1000 : 0) +
-                                     b_ahead2 * 1800;
-                        if (p.n_cta > 256)       // 64 KB of weights per K-block: the weight ring needs the room more than the input ring
-                            score = (long)bn_eff * 100 + (bn >= 256 ? 500 : 0) + (s_in > 3 ? 3 : s_in) * 2500 + s_a * 400 + n_stg * 300 +
-                                    b_ahead2 * 3000;
+                        long score = (long)bn * 100 + (s_in > 4 ? 4 : s_in) * 2500 + s_a * (p.kblocks <= 2 ? 1500 : 400) + n_stg * 2800 +
+                                     (res ? 1000 : 0) + b_ahead2 * 1800;
                         if (p.cs > 1)        // every CTA of the cluster produces operand tiles concurrently: one stage each, plus slack
-                            score = (long)bn_eff * 100 + (bn >= 256 ? 500 : 0) + (s_in > 3 ? 3 : s_in) * 1500 +
-                                    (s_a > p.cs + 1 ? p.cs + 1 : s_a) * 4000 + groups * 2500 + n_stg * 300 + b_ahead2 * 2500;
-                        if (bn < 64 && bn < bn_top) {                        // narrow MMAs are a last resort
-                            if (!allow_narrow) continue;
-                            score -= 20000;
-                        }
+                            score = (long)bn * 100 + (s_in > 3 ? 3 : s_in) * 1500 + (s_a > p.cs + 1 ? p.cs + 1 : s_a) * 4000 + n_stg * 2800 +
+                                    b_ahead2 * 2500;
                         if (score > best) {
                             found = true; best = score;
-                            p.s_a = s_a; p.n_stg = n_stg; p.epi_groups = groups; p.s_in = s_in; p.s_b = s_b; p.bn = bn; p.b_resident = res;
+                            p.s_a = s_a; p.n_stg = n_stg; p.s_in = s_in; p.s_b = s_b; p.bn = bn; p.b_resident = res;
                         }
                     }
-                if (bn <= 16) break;
             }
         }
     if (!found) return false;
     p.nb = (p.n_cta + p.bn - 1) / p.bn;
     p.b_stage_bytes = p.bn * 128;
     p.smem_bytes = p.s_a * kPlanAStage + p.s_b * p.b_stage_bytes + p.s_in * p.in_stage_stride + p.n_stg * kPlanStg + fixed;
-    // both epilogue groups drain every item together, alternating 64-column blocks, whenever there are at least two
-    // blocks: same throughput as taking alternate items, half the exposed drain after a CTA's last item
-    p.epi_colsplit = (!q.head && p.epi_groups == 2 && p.n_cta > 64 && (!q.no_colsplit || p.nacc == 1)) ? 1 : 0;
-    // only one staging tile fits (stride-2 blocks): all eight warps share it, each TMEM lane quarter's two warps split the
-    // block's 64 columns -- these blocks were bound by a single four-warp group draining 3 400 cycles per block
-    p.epi_wide = (!q.head && p.epi_groups == 1 && !q.no_wide) ? 1 : 0;
     return true;
 }
 
@@ -132,7 +108,7 @@ inline int plan_dw_teams(const BlockPlanIn& q, const BlockPlanOut& p) {
 
 inline BlockPlanOut plan_block(const BlockPlanIn& q) {
     BlockPlanOut p{};
-    const long sms = q.n_sms > 0 ? q.n_sms : 148;
+    const long sms = q.n_sms > 0 ? q.n_sms : 132;
     const int NI = q.tile ? 2 : 1, TH = 8, TW = q.tile ? 8 : 16;
     const int IH = (TH - 1) * q.stride + q.ksize, IW = (TW - 1) * q.stride + q.ksize;
     p.kblocks = (q.c_in + kPlanKblk - 1) / kPlanKblk;
@@ -141,14 +117,17 @@ inline BlockPlanOut plan_block(const BlockPlanIn& q) {
     p.dwp_bytes = q.ksize * q.ksize * 128 + 512;
     p.in_stage_stride = (p.in_stage_bytes + p.dwp_bytes + 127) / 128 * 128;
     // Split the output channels into items (each item recomputes the depthwise half for its 128 pixels and reloads the
-    // input tile, so splitting is not free).  Candidates: n_cta <= 512 (the whole TMEM as one accumulator; <= 256 leaves
-    // room for two and overlaps the next item's MMAs with this item's drain), multiples of 64 when there is more than
-    // one split (the epilogue moves whole [128 px][64 ch] tiles and must not touch a neighbouring split's columns).
+    // input tile, so splitting is not free).  Candidates: n_cta <= 128 (the register accumulators), multiples of 64 when there
+    // is more than one split (the epilogue moves whole [128 px][64 ch] tiles and must not touch a neighbouring split's columns).
     // Candidates are tried in the order of their modelled kernel time
-    //     rounds over the SMs x K-blocks x max(depthwise, MMA, L2 -> SM operand traffic) + exposed drain of the last item
-    // until one fits shared memory.  Per-K-block cycles are measured ones (profiles/r01_trace_*); the operand-traffic term
-    // is chip-wide: the L2 delivers ~6300 B/clk to all SMs together (B300_MICROARCH.md), ~5500 sustained here, and the
-    // 14x14 blocks sit on it (conv7: 148 CTAs x 57 KB per K-block every 1750 cycles).
+    //     rounds over the SMs x (K-blocks x max(depthwise, MMA, L2 -> SM operand traffic) + epilogue of the item)
+    // until one fits shared memory.  The per-K-block terms are estimates from H100 figures, not measurements:
+    //   depthwise  k*k taps x 64 channels x 128 pixels on the 128 fp32 lanes of an SM, doubled for the loads, conversions
+    //              and stores that issue beside the FMAs;
+    //   MMA        128 x n_cta x 64 MACs at 2048 dense 16-bit MAC/clk per SM (989 TFLOP/s over 132 SMs at 1.83 GHz);
+    //   L2 -> SM   the input tile and the weight stage of every active CTA at ~3000 B/clk for the whole chip (about 5.5 TB/s);
+    //   epilogue   ~8 cycles per output channel of the item (registers -> staging tile -> TMA store, not overlapped with the
+    //              item's MMAs), plus ~100 cycles of hand-shakes per K-block.
     const int cout_pad = (q.c_out + 15) / 16 * 16;
     struct Cand { long t; int sp, nc, cs; };
     Cand cands[12];
@@ -156,35 +135,30 @@ inline BlockPlanOut plan_block(const BlockPlanIn& q) {
     if (cout_pad <= 64 || q.head) {
         cands[n_cands++] = Cand{0, 1, cout_pad, 1};
     } else {
-        const long dw_c = q.ksize == 5 ? 2100 : (q.stride == 2 ? 1200 : 1000);
-        for (int n_cta = 512; n_cta >= 64; n_cta -= 64) {
+        const long dw_c = 2L * q.ksize * q.ksize * 64;
+        for (int n_cta = kPlanMaxNcta; n_cta >= 64; n_cta -= 64) {
             int sp = (cout_pad + n_cta - 1) / n_cta, nc = n_cta;
             if (sp == 1) nc = cout_pad;                              // a single split needs no 64-alignment
-            if (sp == 1 && cout_pad > 512) continue;
+            if (sp == 1 && cout_pad > kPlanMaxNcta) continue;
             if (sp == 1 && n_cta - 64 >= cout_pad) continue;         // same plan as the next smaller candidate
-            if (q.max_n_cta > 0 && nc > q.max_n_cta && !(sp == 1 && cout_pad <= 256)) continue;
+            if (q.max_n_cta > 0 && nc > q.max_n_cta && !(sp == 1 && cout_pad <= kPlanMaxNcta)) continue;
             const long items = (long)q.n_tiles * sp;
-            // one accumulator cannot overlap an item's MMAs with the previous item's drain: only where every CTA has one item
-            if (nc > 256 && items > sms) continue;
             const long rounds = (items + sms - 1) / sms;
             const long active = items < sms ? items : sms;
-            const long mma_c = 2L * nc;                              // 128 x nc x 64 MACs at 4096 MAC/clk
-            const long l2_c = active * (p.in_stage_bytes + 128L * nc) / 5500;
+            const long mma_c = 4L * nc;
+            const long l2_c = active * (p.in_stage_bytes + 128L * nc) / 3000;
             long kb_c = dw_c > mma_c ? dw_c : mma_c;
             if (l2_c > kb_c) kb_c = l2_c;
-            const long drain = (nc > 64 ? 23L : 45L) * nc;           // two epilogue groups share an item's column blocks
-            const long t = rounds * p.kblocks * (kb_c + 100) + drain;
+            const long t = rounds * (p.kblocks * (kb_c + 100) + 8L * nc);
             int at = n_cands++;
             while (at > 0 && cands[at - 1].t > t) { cands[at] = cands[at - 1]; --at; }
             cands[at] = Cand{t, sp, nc, 1};
         }
-        // Cluster mode: cs CTAs share one tile.  Without it every output-channel split recomputes the whole depthwise half
-        // (conv13: 4 splits x 16 K-blocks of depthwise per CTA against 8 K-blocks' worth of MMA time); with it the depthwise
-        // work of a tile is divided by cs and the K loop runs at the MMA's pace.
-        // Measured (profiles/r02_cluster_ab.txt, stock and pruned widths at batch 64): the hand-over latency and the start-up of a
-        // cluster eat the gain everywhere except on the 7x7 maps with a 5x5 depthwise (decode_conv1: 36.1 -> 32.2 us; the
-        // 3x3 blocks there stay paced by their weight stream), so the automatic choice is limited to that case; the plan
-        // option / FD_TC_CLUSTER = 2 | 4 forces it wherever the block admits it (the bitwise tests do).
+        // Cluster mode: cs CTAs share one tile.  Without it every output-channel split recomputes the whole depthwise half;
+        // with it the depthwise work of a tile is divided by cs and the K loop runs at the MMA's pace, at the price of the
+        // operand hand-over and the cluster's start-up.  The automatic choice is limited to the 7x7 maps with a 5x5 depthwise,
+        // where the depthwise half is the largest share of a K-block; the plan option / FD_TC_CLUSTER = 2 | 4 forces it
+        // wherever the block admits it (the bitwise tests do).
         for (int cs = 2; cs <= 4 && q.cluster != 1; cs *= 2) {
             if (q.cluster > 1 && q.cluster != cs) continue;
             if (q.cluster == 0 && !(q.ksize == 5 && q.tile == 1 && cs == 4)) continue;
@@ -193,16 +167,15 @@ inline BlockPlanOut plan_block(const BlockPlanIn& q) {
             // the instrumented build does not show); the single-wave case is the one the cost model wants anyway
             if ((long)q.n_tiles * cs > sms && !q.cluster_multiwave) continue;
             const int nc = ((cout_pad + cs - 1) / cs + 63) / 64 * 64;
-            if (nc > 256 || nc * (cs - 1) >= cout_pad || p.kblocks < cs) continue;      // every CTA owns >= 1 K-block and a non-empty split
+            if (nc > kPlanMaxNcta || nc * (cs - 1) >= cout_pad || p.kblocks < cs) continue;      // every CTA owns >= 1 K-block and a non-empty split
             const long n_cl = sms / cs;
             const long rounds = ((long)q.n_tiles + n_cl - 1) / n_cl;
-            const long mma_c = 2L * nc;
+            const long mma_c = 4L * nc;
             const long active = (q.n_tiles < n_cl ? q.n_tiles : n_cl) * cs;
-            const long l2_c = active * (p.in_stage_bytes / cs + 128L * nc) / 5500;
+            const long l2_c = active * (p.in_stage_bytes / cs + 128L * nc) / 3000;
             long kb_c = dw_c / cs > mma_c ? dw_c / cs : mma_c;
             if (l2_c > kb_c) kb_c = l2_c;
-            const long drain = (nc > 64 ? 23L : 45L) * nc;
-            long t = rounds * p.kblocks * (kb_c + 150) + drain + 1500;                   // + cluster start-up and hand-over latency
+            long t = rounds * (p.kblocks * (kb_c + 150) + 8L * nc) + 1500;               // + estimated cluster start-up and hand-over
             if (q.cluster > 1) t = -1;                                                   // forced
             int at = n_cands++;
             while (at > 0 && cands[at - 1].t > t) { cands[at] = cands[at - 1]; --at; }
@@ -213,19 +186,7 @@ inline BlockPlanOut plan_block(const BlockPlanIn& q) {
         p.splits = cands[i].sp; p.n_cta = cands[i].nc; p.cs = cands[i].cs;
         p.items = q.n_tiles * p.splits;
         p.cpad_all = p.n_cta * p.splits;
-        p.nacc = p.n_cta > 256 ? 1 : 2;
-        p.tmem_cols = 32;
-        while (p.tmem_cols < p.nacc * p.n_cta) p.tmem_cols *= 2;
-        if (plan_block_smem(q, p, false)) { p.ok = 1; p.dw_teams = plan_dw_teams(q, p); return p; }
-    }
-    for (int i = 0; i < n_cands; ++i) {                              // nothing fits with full-width MMAs: accept narrow ones
-        p.splits = cands[i].sp; p.n_cta = cands[i].nc; p.cs = cands[i].cs;
-        p.items = q.n_tiles * p.splits;
-        p.cpad_all = p.n_cta * p.splits;
-        p.nacc = p.n_cta > 256 ? 1 : 2;
-        p.tmem_cols = 32;
-        while (p.tmem_cols < p.nacc * p.n_cta) p.tmem_cols *= 2;
-        if (plan_block_smem(q, p, true)) { p.ok = 1; p.dw_teams = plan_dw_teams(q, p); return p; }
+        if (plan_block_smem(q, p)) { p.ok = 1; p.dw_teams = plan_dw_teams(q, p); return p; }
     }
     p.ok = 0;
     return p;

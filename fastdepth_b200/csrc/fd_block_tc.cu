@@ -1,30 +1,25 @@
-// Fused depthwise -> pointwise block kernel for sm_100a (tcgen05 + TMEM + TMA), persistent and
+// Fused depthwise -> pointwise block kernel for sm_90a (wgmma + TMA + mbarrier rings), persistent and
 // warp-specialised.
 //
 // One kernel per conv_dw / decode_conv block (reference imagenet/mobilenet.py:29-38, models.py:61-75,
 // 683-697) including, for decoder blocks, the nearest-x2 upsample and the skip add of models.py:723-729
 // in the epilogue, and optionally decode_conv6 (models.py:698,731) folded below the last upsample.
 //
-// Work item = one tile of 128 output pixels (NI images x TH x TW) times n_cta output channels.  The grid is
-// one CTA per SM; every CTA walks items blockIdx.x, +gridDim.x, ... and all four roles run concurrently on
-// different items / K-blocks:
+// Work item = one tile of 128 output pixels (NI images x TH x TW) times n_cta (<= 128) output channels.  The grid is
+// one CTA per SM; every CTA walks items blockIdx.x, +gridDim.x, ... and the roles run concurrently on different
+// items / K-blocks:
 //   warp 16     TMA producer : per 64-channel K-block, one 4-D box load of the input halo tile
-//                              [NI][IH][IW][64ch] (OOB zero fill == conv zero padding) and the [BN x 64]
+//                              [NI][IH][IW][64ch] (OOB zero fill == conv zero padding) and the [bn x 64]
 //                              slices of the pointwise weights (128B-swizzled, K-major); when the whole weight
 //                              matrix fits it is loaded once and stays resident
-//   warps 0-7   depthwise    : lane = channel pair, 4x4 output pixels per warp; 3x3: FFMA2 on fp32 pairs widened once,
-//                              5x5: FHFMA (16-bit x 16-bit + fp32) -- exact products, fp32 accumulation either way ->
-//                              BN affine (FFMA2) -> act folded into the 16-bit conversion -> written straight into the
+//   warps 8-15  depthwise    : lane = channel pair, 4x4 output pixels per warp, exact 16-bit products accumulated in fp32 ->
+//                              BN affine -> act folded into the 16-bit conversion -> written straight into the
 //                              128B-swizzled K-major A operand tile in shared memory (never touches HBM)
-//   warp 17     MMA issuer   : tcgen05.mma.cta_group::1.kind::f16, M=128, N<=256 per instruction, K=16, fp32 accumulators
-//                              in TMEM: two of <= 256 columns (the next item's MMAs overlap this item's drain) or one
-//                              of up to 512 (a whole 512-channel output tile as ONE item)
-//   warps 8-15  epilogue     : tcgen05.ld 32x32b -> BN affine + act -> 16-bit -> staging tile -> TMA tensor stores (x4
-//                              strided views for the nearest-x2 upsample, reduce-add into the skip tensor; or the folded
-//                              1-channel head).  Two groups of four warps: alternate items, or alternate 64-column blocks
-//                              of every item, or all eight warps on one staging tile (see TcParams)
-// mbarrier rings: input stages (TMA -> dw), A stages (dw -> MMA), B stages (TMA -> MMA), accumulators
-// (MMA -> epilogue).
+//   warps 0-7   consumers    : two warpgroups, each owning 64 of the tile's 128 pixel rows: wgmma m64n64k16 (fp32
+//                              accumulators in registers) over the K-blocks, then BN affine + act -> 16-bit -> staging
+//                              tile -> TMA tensor stores (x4 strided views for the nearest-x2 upsample, reduce-add into
+//                              the skip tensor; or the folded 1-channel head)
+// mbarrier rings: input stages (TMA -> dw), A stages (dw -> wgmma), B stages (TMA -> wgmma).
 #include <cuda.h>
 
 #include <cstdio>
@@ -39,20 +34,15 @@
 namespace fd {
 
 constexpr int TC_DW_WARPS = 8;
-constexpr int TC_EPI_WARPS = 8;
-// Which role gets the LOW warp ids matters: the warp schedulers favour them when several warps are ready, and the epilogue
-// warps (few instructions, long dependent chains: TMEM load -> affine -> store -> fence -> barrier) were being starved by the
-// FMA streams of the depthwise warps.  Epilogue on warps 0..7: whole forward 610 -> 594 us (conv2 51 -> 46 us, conv1 58 -> 55 us).
-#ifdef FD_TC_DW_FIRST         // build-time A/B: the round-1 order
-constexpr int TC_WARP_EPI0 = TC_DW_WARPS, TC_WARP_DW0 = 0;   // depthwise 0..7, epilogue 8..15 (warp % 4 == TMEM lane quarter)
-#else
-constexpr int TC_WARP_EPI0 = 0, TC_WARP_DW0 = TC_EPI_WARPS;  // epilogue 0..7 (warp % 4 == TMEM lane quarter), depthwise 8..15
-#endif
+constexpr int TC_EPI_WARPS = 8;                              // two consumer warpgroups (wgmma + epilogue)
+// consumers on warps 0..7 (warpgroups 0 and 1), depthwise on 8..15; TcParams::epi_high swaps the two groups (both stay
+// warpgroup-aligned, as wgmma requires)
+constexpr int TC_WARP_EPI0 = 0, TC_WARP_DW0 = TC_EPI_WARPS;
 constexpr int TC_WARP_TMA = TC_DW_WARPS + TC_EPI_WARPS;      // 16
-constexpr int TC_WARP_MMA = TC_WARP_TMA + 1;                 // 17
-constexpr int TC_THREADS = (TC_WARP_MMA + 1) * 32;           // 576
-constexpr int TC_WARP_BCAST = TC_WARP_MMA + 1;               // 18: cluster mode only -- hands finished operand tiles to the peer CTAs
-constexpr int TC_THREADS_CL = (TC_WARP_BCAST + 1) * 32;      // 608 (19 warps x 96 registers still fit the register file)
+constexpr int TC_THREADS = (TC_WARP_TMA + 1) * 32;           // 544
+constexpr int TC_WARP_BCAST = TC_WARP_TMA + 1;               // 17: cluster mode only -- hands finished operand tiles to the peer CTAs
+constexpr int TC_THREADS_CL = (TC_WARP_BCAST + 1) * 32;      // 576
+constexpr int TC_NCH = 2;                                    // 64-column accumulator blocks per item (n_cta <= 128)
 constexpr int TC_KBLK = 64;                     // channels per K-block (one 128-byte swizzle row)
 constexpr int TC_A_STAGE_BYTES = 128 * 128;     // 128 rows x 64 x 2 B
 constexpr int TC_MAX_IN = 6, TC_MAX_A = 6, TC_MAX_B = 16;
@@ -66,13 +56,11 @@ struct TcParams {
     int kblocks;          // ceil(c_in / 64)
     int cin_pad;          // kblocks * 64
     int n_cta;            // output channels per item (multiple of 16)
-    int bn;               // B sub-block width (columns per tcgen05.mma), multiple of 16, <= 256
+    int bn;               // B sub-block width: 64 or 128 rows of the weight matrix per stage (rows past c_out load as zeros)
     int nb;               // sub-blocks per K-block = ceil(n_cta / bn)
     int s_in, s_a, s_b;   // pipeline depths
     int b_resident;       // 1: all kblocks*nb weight blocks are loaded once and kept (s_b == kblocks*nb)
-    int nacc;             // TMEM accumulator buffers (2 when 2*n_cta <= 512)
     int in_stage_bytes, b_stage_bytes;
-    int tmem_cols;        // power of two >= 32, >= nacc * n_cta
     int act, upsample;
     int head;             // 1: fold the C->1 head (writes head_out instead of out)
     int head_act;
@@ -83,17 +71,11 @@ struct TcParams {
     int in_stage_stride;  // in_stage_bytes + dw parameter block, rounded to 128
     int dwp_bytes;        // bytes of one K-block's depthwise parameter block
     int cpad_all;         // n_cta * splits: padded length of the pointwise BN vectors
-    int n_stg;            // epilogue staging tiles (16 KB each) in total: epi_groups x (2 or 1)
-    int epi_colsplit;     // 1: both epilogue groups drain EVERY item, group g taking the 64-column blocks g, g+2, ... (halves the
-                          //    exposed drain after a CTA's last item; needed when one 512-column accumulator is all there is)
-    int epi_wide;         // 1 (with epi_groups == 1): all eight epilogue warps work on ONE staging tile, the two warps of a TMEM
-                          //    lane quarter taking 32 of each block's 64 columns -- twice the drain rate where only one tile fits
-    int epi_groups;       // 2: two groups of four epilogue warps take alternate items; 1: one group takes all (smem is tight)
+    int n_stg;            // epilogue staging tiles (16 KB each): with two, one tile's TMA store overlaps filling the other
     int out_pitch, skip_pitch;   // elements between pixels of the output / skip tensors (>= c_out: channel slice of a concat buffer)
-    int sleep_ns;         // > 0: latency-tolerant waits (epilogue: accumulator ready, TMA producer: stage free) back off with
-                          //      nanosleep between probes instead of re-issuing try_wait every ~27 cycles (those probes are real
-                          //      issue slots: a third of all warp instructions of decode_conv5 in the round-1 capture)
-    int mma_sleep_ns;     // same for the MMA issuer's waits (operand ready / accumulator drained)
+    int sleep_ns;         // > 0: latency-tolerant waits (TMA producer: stage free) back off with nanosleep between probes
+                          //      instead of re-issuing try_wait (those probes take issue slots from the depthwise warps)
+    int mma_sleep_ns;     // same for the consumers' waits for an operand stage
     int dw_sleep_ns;      // same for the depthwise warps' wait for an input stage
     int epi_tma;          // 1: staging tiles leave through TMA tensor stores (4 strided views for nearest-x2 upsampling)
     int epi_red;          // 1: ... as element-wise ADD into the skip tensor, which then IS the block's output (in place)
@@ -103,9 +85,7 @@ struct TcParams {
     const float* head_w;  // [cpad_all]
     int dw_teams;         // 2: the depthwise warps form two teams of four that take alternate K-block steps, two 4x4 blocks per warp
                           // (needs even s_in and s_a); 1: eight warps in lock-step, one block each
-    int epi_high;         // 1: the epilogue runs on warps 8..15 and the depthwise on 0..7 (default: the other way round).  Which role
-                          // the schedulers' arbitration should favour depends on which one paces the block: the stride-2 blocks are
-                          // paced by their single epilogue staging tile, the others by the depthwise
+    int epi_high;         // 1: the consumers run on warps 8..15 and the depthwise on 0..7 (default: the other way round)
     int wmc;              // weight-multicast cluster size (1, 2, 4): the wmc CTAs of a cluster take wmc consecutive tiles with the SAME
                           // output-channel split and each loads 1/wmc of every weight block, TMA-multicast into all of them
     int cs;               // cluster size (1, 2, 4): the cs CTAs of a cluster work on the SAME tile (splits == cs); CTA r computes the
@@ -119,11 +99,8 @@ struct TcBarriers {
     uint64_t in_full[TC_MAX_IN], in_empty[TC_MAX_IN];
     uint64_t a_full[TC_MAX_A], a_empty[TC_MAX_A];
     uint64_t b_full[TC_MAX_B], b_empty[TC_MAX_B];
-    uint64_t acc_full[2], acc_empty[2];
     uint64_t aff_full;    // the pointwise BN affine has landed in shared memory (one bulk copy issued in the prologue)
     uint64_t dw_done[4];  // cluster mode: the depthwise warps have finished (and proxy-fenced) an operand tile -> broadcast thread
-    uint32_t tmem_base;
-    uint32_t pad;
 };
 
 struct ItemCoord { int img0, oy0, ox0, n0; };
@@ -207,11 +184,10 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
         const uint32_t dw_arrivals = (uint32_t)(TC_DW_WARPS / ((CL || p.dw_teams != 2) ? 1 : 2));     // warps that work on one K-block step
         for (int i = 0; i < TC_MAX_IN; ++i) { mbar_init(smem_u32(&bars->in_full[i]), 1); mbar_init(smem_u32(&bars->in_empty[i]), dw_arrivals); }
         // cluster mode: an A stage is full after ONE arrival (the owner's broadcast thread, or this CTA's own expect_tx for a
-        // tile that arrives by bulk copy) and free again when the MMA streams of all cs CTAs have committed past it
-        for (int i = 0; i < TC_MAX_A; ++i) { mbar_init(smem_u32(&bars->a_full[i]), CL ? 1u : dw_arrivals); mbar_init(smem_u32(&bars->a_empty[i]), cs); }
+        // tile that arrives by bulk copy) and free again when both consumer warpgroups of all cs CTAs are done reading it
+        for (int i = 0; i < TC_MAX_A; ++i) { mbar_init(smem_u32(&bars->a_full[i]), CL ? 1u : dw_arrivals); mbar_init(smem_u32(&bars->a_empty[i]), 2u * cs); }
         for (int i = 0; i < 4; ++i) mbar_init(smem_u32(&bars->dw_done[i]), TC_DW_WARPS);
-        for (int i = 0; i < TC_MAX_B; ++i) { mbar_init(smem_u32(&bars->b_full[i]), 1); mbar_init(smem_u32(&bars->b_empty[i]), wmc); }   // multicast: freed by all
-        for (int i = 0; i < 2; ++i) { mbar_init(smem_u32(&bars->acc_full[i]), 1); mbar_init(smem_u32(&bars->acc_empty[i]), (p.epi_colsplit || p.epi_wide) ? TC_EPI_WARPS : TC_EPI_WARPS / 2); }
+        for (int i = 0; i < TC_MAX_B; ++i) { mbar_init(smem_u32(&bars->b_full[i]), 1); mbar_init(smem_u32(&bars->b_empty[i]), 2u * wmc); }   // multicast: freed by all
         mbar_init(smem_u32(&bars->aff_full), 1);
         fence_barrier_init();
         // the pointwise BN affine (constant data, independent of the previous kernel) comes in as ONE asynchronous bulk copy that the
@@ -226,7 +202,6 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                smem_u32(&bars->a_empty[0]), smem_u32(&bars->b_full[0]), smem_u32(&bars->b_empty[0]), smem_u32(&bars->acc_full[0]), smem_u32(&bars->acc_empty[0]),
                smem_u32(&bars->dw_done[0]));
 #endif
-    if (warp == TC_WARP_MMA) tmem_alloc(smem_u32(&bars->tmem_base), (uint32_t)p.tmem_cols);     // MMA warp owns TMEM
     if (warp == TC_WARP_TMA && lane == 0) {
         tma_prefetch_desc(&tm_in);
         tma_prefetch_desc(&tm_w);
@@ -243,11 +218,8 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
     }
     pdl_launch_dependents();                       // the next kernel may begin its own prologue
     pdl_wait_prior_grid();                         // everything below reads what the previous kernel wrote
-    tc_fence_before();
     if constexpr (CLM != 0) cluster_sync_all();    // every CTA's barriers exist before a peer may signal or copy into them
     else __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = bars->tmem_base;
 
     if (warp == TC_WARP_TMA) {
         // =========================== TMA producer ===========================
@@ -298,81 +270,6 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                             tma_load_2d(smem_base + b_off + sb * p.b_stage_bytes, &tm_w, smem_u32(&bars->b_full[sb]), kb * TC_KBLK,
                                         n0 + nbi * p.bn);
                     }
-            }
-        }
-    } else if (warp == TC_WARP_MMA) {
-        // =========================== MMA issuer ===========================
-        // A single thread drives the tensor core; every instruction on this path is serial latency for the whole
-        // CTA, so descriptors are pre-split (constant high word) and advanced with 32-bit adds only.
-        if (lane == 0) {
-            const uint32_t idesc_base = (1u << 4) | (MF::kUmmaFormat << 7) | (MF::kUmmaFormat << 10) | ((128u >> 4) << 24);
-            const uint32_t idesc_full = idesc_base | ((uint32_t)(p.bn >> 3) << 17);
-            const uint32_t idesc_last = idesc_base | ((uint32_t)((p.n_cta - (p.nb - 1) * p.bn) >> 3) << 17);
-            const uint32_t a_lo0 = sw128_desc_lo(smem_base + a_off), b_lo0 = sw128_desc_lo(smem_base + b_off);
-            const uint32_t a_step = TC_A_STAGE_BYTES >> 4, b_step = (uint32_t)p.b_stage_bytes >> 4;
-            const uint32_t bar_a_full = smem_u32(&bars->a_full[0]), bar_a_empty = smem_u32(&bars->a_empty[0]);
-            const uint32_t bar_b_full = smem_u32(&bars->b_full[0]), bar_b_empty = smem_u32(&bars->b_empty[0]);
-            const uint32_t bar_acc_full = smem_u32(&bars->acc_full[0]), bar_acc_empty = smem_u32(&bars->acc_empty[0]);
-            Ring ra, rb, racc;
-            int tr = 0;
-            bool first = true;
-            // cluster mode: operand tiles of K-blocks another CTA owns arrive by bulk copy; this thread arms a stage's barrier with
-            // the expected bytes for its NEXT use as soon as the current use has been observed complete (kb_arm = K-block of that
-            // next use, q_left = K-block uses of this CTA's whole run that are not armed yet)
-            int kb_arm = 0;
-            long q_left = 0;
-            const uint16_t cl_mask = (uint16_t)((1u << cs) - 1u), cl_mask_w = (uint16_t)((1u << wmc) - 1u);
-            if constexpr (CL) {
-                const int n_it = u_first < u_count ? (u_count - 1 - u_first) / u_stride + 1 : 0;
-                q_left = (long)n_it * p.kblocks;
-                for (int s = 0; s < p.s_a && q_left > 0; ++s, --q_left) {
-                    if ((uint32_t)kb_arm % cs != crank) mbar_expect_tx(bar_a_full + 8u * (uint32_t)s, (uint32_t)TC_A_STAGE_BYTES);
-                    if (++kb_arm == p.kblocks) kb_arm = 0;
-                }
-            }
-            for (int u = u_first; u < u_count; u += u_stride, racc.next((uint32_t)p.nacc), first = false) {
-                mbar_wait_sleep_sel<kHint>(bar_acc_empty + 8u * racc.s, racc.ph ^ 1u, (uint32_t)p.mma_sleep_ns);   // epilogue has drained this accumulator
-                const uint32_t d_tmem = tmem_base + racc.s * (uint32_t)p.n_cta;
-                for (int kb = 0; kb < p.kblocks; ++kb, ra.next((uint32_t)p.s_a)) {
-                    mbar_wait_sleep_sel<kHint>(bar_a_full + 8u * ra.s, ra.ph, (uint32_t)p.mma_sleep_ns);
-                    if constexpr (CL) {
-                        if (q_left > 0) {
-                            if ((uint32_t)kb_arm % cs != crank) mbar_expect_tx(bar_a_full + 8u * ra.s, (uint32_t)TC_A_STAGE_BYTES);
-                            if (++kb_arm == p.kblocks) kb_arm = 0;
-                            --q_left;
-                        }
-                    }
-                    tc_fence_after();
-                    TC_TRACE(4, tr);
-                    const uint32_t a_lo = a_lo0 + ra.s * a_step;
-                    for (int nbi = 0; nbi < p.nb; ++nbi) {
-                        uint32_t sb;
-                        if (p.b_resident) {
-                            sb = (uint32_t)(kb * p.nb + nbi);
-                            if (first) { mbar_wait_sel<kHint>(bar_b_full + 8u * sb, 0); tc_fence_after(); }
-                        } else {
-                            sb = rb.s;
-                            mbar_wait_sel<kHint>(bar_b_full + 8u * sb, rb.ph);
-                            rb.next((uint32_t)p.s_b);
-                            tc_fence_after();
-                        }
-                        const uint32_t b_lo = b_lo0 + sb * b_step;
-                        const uint32_t idesc = (nbi == p.nb - 1) ? idesc_last : idesc_full;
-                        const uint32_t dcol = d_tmem + (uint32_t)(nbi * p.bn);
-                        umma_f16_lohi(dcol, a_lo, b_lo, kSw128DescHi, idesc, kb > 0 ? 1u : 0u);
-                        umma_f16_lohi(dcol, a_lo + 2, b_lo + 2, kSw128DescHi, idesc, 1u);     // +32 B (16 elements) per K step
-                        umma_f16_lohi(dcol, a_lo + 4, b_lo + 4, kSw128DescHi, idesc, 1u);
-                        umma_f16_lohi(dcol, a_lo + 6, b_lo + 6, kSw128DescHi, idesc, 1u);
-                        if (!p.b_resident) {
-                            if constexpr (CW) umma_commit_multicast(bar_b_empty + 8u * sb, cl_mask_w);   // the stage is refilled for all CTAs at once
-                            else umma_commit(bar_b_empty + 8u * sb);
-                        }
-                    }
-                    if constexpr (CL) umma_commit_multicast(bar_a_empty + 8u * ra.s, cl_mask);    // frees the stage in every CTA's count
-                    else umma_commit(bar_a_empty + 8u * ra.s);
-                    TC_TRACE(5, tr); ++tr;
-                }
-                umma_commit(bar_acc_full + 8u * racc.s);
             }
         }
     } else if (CL && warp == TC_WARP_BCAST) {
@@ -434,18 +331,14 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                 // the proxy fence at the end (a MEMBAR.ALL.CTA, ~36 cycles per store still in flight) finds few pending
                 mbar_wait_sel<kHint>(smem_u32(&bars->a_empty[sa]), pha ^ 1u);
                 uint8_t* a_s = smem + a_off + sa * TC_A_STAGE_BYTES;
-#ifdef FD_DW3_FHFMA                      // build-time A/B switch: 3x3 depthwise on FHFMA like the 5x5 (measured 1.2 % slower end to end)
-                constexpr bool kDwFfma2 = false;
-#else
-                constexpr bool kDwFfma2 = KS == 3;
-#endif
+                constexpr bool kDwFfma2 = KS == 3;     // 3x3: taps widened to fp32 pairs once per step; 5x5: widened on use
                 // 5x5: the 25 tap words of the lane's channel pair, once per step (shared by both blocks of a team warp)
                 uint32_t wv[(HALFK || kDwFfma2) ? 1 : KS * KS];
                 if constexpr (!HALFK && !kDwFfma2) {
 #pragma unroll
                     for (int i = 0; i < KS * KS; ++i) wv[i] = *reinterpret_cast<const uint32_t*>(prm + i * 128 + lane * 4);
                 }
-#pragma unroll 1                           // (interleaving a team warp's two blocks, tried for the half-K path: conv1 55.4 -> 60.8 us)
+#pragma unroll 1
                 for (int blk = 0; blk < nblk; ++blk) {
                 const int bidx = member * nblk + blk;                      // 4x4-pixel block of the tile
                 const int ni = bidx / BPI, rem = bidx % BPI, br = rem / BPR, bc = rem % BPR;
@@ -491,11 +384,8 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                         }
                     }
                 } else if constexpr (kDwFfma2) {
-                    // Inner product on FFMA2: every 16-bit word (the lane's channel pair) is widened to an fp32 pair once
-                    // (two HADD2.F32), then ONE two-wide FMA per pixel-tap instead of two FHFMA: 144 FFMA2 + 90 HADD2 against
-                    // 288 FHFMA per 4x4 block.  Bit-identical (a 16-bit x 16-bit product is exact in either FMA); FFMA2 issues
-                    // at well under 0.5 / clk so the FMA pipe time is about the same, the gain is the issue slots: measured
-                    // +1.2 % on the whole forward (conv1 68 -> 64 us).
+                    // Every 16-bit word (the lane's channel pair) is widened to an fp32 pair once, then one fp32 FMA per
+                    // channel and pixel-tap.  A 16-bit x 16-bit product is exact in fp32, so this is the mixed-precision result.
                     f32x2 acc[4][4];
 #pragma unroll
                     for (int a = 0; a < 4; ++a)
@@ -531,9 +421,7 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                         }
                     }
                 } else {
-                    // 5x5 stays on the mixed-precision FHFMA (16-bit x 16-bit + fp32, exact products): tools/fma2_tput5.cu under
-                    // this kernel's register cap gives 2 118 cycles per 4x4 block for 800 FHFMA (~0.76 / clk / scheduler, close
-                    // to full rate) against 2 720 for 400 FFMA2 + 178 HADD2, and in the kernel decode_conv5 went 88 -> 109 us
+                    // 5x5: the 25 tap words stay packed (register budget); MixFma::fma2 widens on use
                     float acc[4][4][2];
 #pragma unroll
                     for (int a = 0; a < 4; ++a)
@@ -577,94 +465,137 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
             }
         }
     } else {
-        // =========================== epilogue warps ===========================
-        // Two independent groups of four warps; group g drains TMEM accumulator g, i.e. every second item, so one
-        // group's TMEM-load / barrier latency overlaps the other group's math and stores.
-        const int ew = rwarp - TC_WARP_EPI0;               // (rwarp and warp agree modulo 4: the TMEM lane quarter is the hardware's)
-        const int q = ew & 3, grp = ew >> 2;               // TMEM lane quarter (== warp % 4), group / accumulator index
-        const int m = q * 32 + lane;                       // accumulator row == pixel of the tile
-        const int e_ni = m / (TH * TW), e_ty = (m / TW) % TH, e_tx = m % TW;
-        const bool wide = p.epi_wide != 0;                 // one group of eight warps, warp pair (w, w+4) splits each block's columns
-        const uint32_t bar_id = wide ? 1u : 1u + (uint32_t)grp;     // named barrier of this group
-        const uint32_t bar_n = wide ? 256u : 128u;                  // ... and its thread count
-        const bool elected = q == 0 && lane == 0 && (!wide || grp == 0);   // issues this group's tensor stores
+        // =========================== consumer warpgroups: wgmma + epilogue ===========================
+        // Warpgroup wg owns pixel rows [64 wg, 64 wg + 64) of every item; a thread holds rows r0 and r0 + 8 of each 64-column
+        // accumulator block (fragment layout: see the wgmma wrappers).  Both warpgroups fill every staging tile together.
+        const int ew = rwarp - TC_WARP_EPI0;               // 0..7 (rwarp = warp ^ 8 keeps the warpgroups intact)
+        const int wg = ew >> 2, wq = ew & 3;
+        const int r0 = wg * 64 + wq * 16 + (lane >> 2), cq = (lane & 3) * 2;
+        const bool leader = wq == 0 && lane == 0;          // releases this warpgroup's operand stages
+        const bool elected = ew == 0 && lane == 0;         // issues the tensor stores (and, in cluster mode, arms the A ring)
+        constexpr uint32_t bar_id = 1u, bar_n = 256u;      // named barrier of the eight consumer warps
         T* __restrict__ outp = reinterpret_cast<T*>(p.out);
         const T* __restrict__ skipp = reinterpret_cast<const T*>(p.skip);
-        const int ngrp = p.epi_groups;                     // 2, or 1 when shared memory is tight (group 1 then idles)
-        const int n_stg_g = p.head ? 0 : p.n_stg / ngrp;   // staging tiles of this group: 1 or 2
-        const uint32_t stg_grp = stg_off + (wide ? 0u : (uint32_t)grp) * (uint32_t)n_stg_g * 16384u;
-        const bool cs = p.epi_colsplit != 0;               // both groups on every item, alternating column blocks
-        uint32_t ab = (ngrp == 2 && !cs) ? (uint32_t)grp : 0u, pa = 0;   // accumulator buffer and its mbarrier phase
+        const int n_stg = p.n_stg < 2 ? 1 : 2;
+        const int nch = (p.n_cta + 63) >> 6;               // 64-column accumulator blocks of an item
+        const int bn_ch = p.bn >> 6;                       // ... per weight stage (1 or 2); nb = nch / bn_ch stages per K-block
+        const uint32_t a_lo0 = sw128_desc_lo(smem_base + a_off + (uint32_t)wg * 8192u), b_lo0 = sw128_desc_lo(smem_base + b_off);
+        const uint32_t a_step = TC_A_STAGE_BYTES >> 4, b_step = (uint32_t)p.b_stage_bytes >> 4;
+        Ring ra, rb;
         int tr = 0;
         uint32_t stg_flip = 0;
+        bool first = true;
+        // cluster mode: operand tiles of K-blocks another CTA owns arrive by bulk copy; the elected thread arms a stage's barrier
+        // with the expected bytes for its NEXT use as soon as the current use has been observed complete (kb_arm = K-block of
+        // that next use, q_left = K-block uses of this CTA's whole run that are not armed yet)
+        int kb_arm = 0;
+        long q_left = 0;
+        if constexpr (CL) {
+            if (elected) {
+                const int n_it = u_first < u_count ? (u_count - 1 - u_first) / u_stride + 1 : 0;
+                q_left = (long)n_it * p.kblocks;
+                for (int s = 0; s < p.s_a && q_left > 0; ++s, --q_left) {
+                    if ((uint32_t)kb_arm % cs != crank) mbar_expect_tx(smem_u32(&bars->a_full[s]), (uint32_t)TC_A_STAGE_BYTES);
+                    if (++kb_arm == p.kblocks) kb_arm = 0;
+                }
+            }
+        }
         mbar_wait_sel<kHint>(smem_u32(&bars->aff_full), 0);      // BN affine in place (bulk copy of the prologue)
-        const int u_step = (cs ? 1 : ngrp) * u_stride;
-        for (int u = u_first + ((cs || wide) ? 0 : grp) * u_stride; (grp < ngrp || wide) && u < u_count; u += u_step) {
+        for (int u = u_first; u < u_count; u += u_stride, first = false) {
             const int w = item_of(u);
             const ItemCoord c = decode_item(p, w, NI, TH, TW);
-            const int img = c.img0 + e_ni, oy = c.oy0 + e_ty, ox = c.ox0 + e_tx;
-            const bool valid = img < p.n && oy < p.h_out && ox < p.w_out;
-            mbar_wait_sleep_sel<kHint>(smem_u32(&bars->acc_full[ab]), pa, (uint32_t)p.sleep_ns);
-            tc_fence_after();
-            if (grp == 0 && elected) TC_TRACE(6, tr);
-            const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16) + ab * (uint32_t)p.n_cta;
+            float acc[TC_NCH][32];
+#pragma unroll
+            for (int j = 0; j < TC_NCH; ++j)
+#pragma unroll
+                for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+            for (int kb = 0; kb < p.kblocks; ++kb, ra.next((uint32_t)p.s_a)) {
+                mbar_wait_sleep_sel<kHint>(smem_u32(&bars->a_full[ra.s]), ra.ph, (uint32_t)p.mma_sleep_ns);
+                if constexpr (CL) {
+                    if (elected && q_left > 0) {
+                        if ((uint32_t)kb_arm % cs != crank) mbar_expect_tx(smem_u32(&bars->a_full[ra.s]), (uint32_t)TC_A_STAGE_BYTES);
+                        if (++kb_arm == p.kblocks) kb_arm = 0;
+                        --q_left;
+                    }
+                }
+                if (elected) TC_TRACE(4, tr);
+                uint32_t sbs[TC_NCH] = {0u, 0u};                  // weight stage of each 64-column block
+                for (int nbi = 0; nbi * bn_ch < nch; ++nbi) {
+                    uint32_t sb;
+                    if (p.b_resident) {
+                        sb = (uint32_t)(kb * (nch / bn_ch) + nbi);
+                        if (first) mbar_wait_sel<kHint>(smem_u32(&bars->b_full[sb]), 0);
+                    } else {
+                        sb = rb.s;
+                        mbar_wait_sel<kHint>(smem_u32(&bars->b_full[sb]), rb.ph);
+                        rb.next((uint32_t)p.s_b);
+                    }
+                    sbs[nbi] = sb;
+                }
+                const uint32_t a_lo = a_lo0 + ra.s * a_step;
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < TC_NCH; ++j) {
+                    if (j < nch) {
+                        const uint32_t b_lo = b_lo0 + (bn_ch == 2 ? sbs[0] * b_step + (uint32_t)j * 512u : sbs[j] * b_step);
+#pragma unroll
+                        for (int k4 = 0; k4 < 4; ++k4)        // +32 B (16 elements) per K step
+                            wgmma_n64<T>(acc[j], sw128_desc(a_lo + 2u * k4), sw128_desc(b_lo + 2u * k4), (kb > 0 || k4 > 0) ? 1u : 0u);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait0();
+                if (leader) {                                    // this warpgroup is done reading the stages
+                    const uint32_t bar_a = smem_u32(&bars->a_empty[ra.s]);
+                    if constexpr (CL) { for (uint32_t r = 0; r < cs; ++r) mbar_arrive_cluster(mapa_u32(bar_a, r)); }
+                    else mbar_arrive(bar_a);
+                    if (!p.b_resident)
+                        for (int nbi = 0; nbi * bn_ch < nch; ++nbi) {
+                            const uint32_t bar_b = smem_u32(&bars->b_empty[sbs[nbi]]);
+                            if constexpr (CW) { for (uint32_t r = 0; r < wmc; ++r) mbar_arrive_cluster(mapa_u32(bar_b, r)); }
+                            else mbar_arrive(bar_b);
+                        }
+                }
+                if (elected) { TC_TRACE(5, tr); ++tr; }
+            }
 
             if (!p.head) {
                 // per block of 64 output channels:
-                //  A: TMEM -> BN affine + act -> 16-bit -> shared staging tile [128 pixels][64 ch] (16-byte chunks XOR-swizzled
+                //  A: registers -> BN affine + act -> 16-bit -> shared staging tile [128 pixels][64 ch] (16-byte chunks XOR-swizzled
                 //     exactly like a SWIZZLE_128B tensor-map box)
-                //  B: the tile leaves through TMA tensor stores (or, as a fallback, coalesced 16-byte LSU stores)
-                const int nblk = (p.n_cta + 63) >> 6;
+                //  B: the tile leaves through TMA tensor stores (or coalesced 16-byte LSU stores)
                 const float2* aff = s_pw_affine + c.n0;                  // this item's BN affine, 8 bytes per channel
-                const int cb_step = cs ? 2 : 1;
-                const int cb_last = cs ? ((nblk - 1 - grp) & ~1) + grp : nblk - 1;     // this group's last block of the item
-                for (int cb = cs ? grp : 0; cb < nblk; cb += cb_step) {
-                    uint8_t* stg = smem + stg_grp + (n_stg_g == 2 ? (stg_flip & 1u) * 16384u : 0u);
+#pragma unroll
+                for (int cb = 0; cb < TC_NCH; ++cb) {
+                    if (cb >= nch) break;
+                    uint8_t* stg = smem + stg_off + (n_stg == 2 ? (stg_flip & 1u) * 16384u : 0u);
                     ++stg_flip;
-                    if (n_stg_g == 1 && stg_flip > 1) {                  // single staging buffer: wait until it is free again
+                    if (n_stg == 1 && stg_flip > 1) {                    // single staging buffer: wait until it is free again
                         if (p.epi_tma && elected) bulk_wait_read0();
                         asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");
                     }
-                    uint8_t* row = stg + m * 128;
 #pragma unroll
-                    for (int half = 0; half < 2; ++half) {
-                        const int col0 = cb * 64 + half * 32;             // first accumulator column of this half block
-                        if (col0 < p.n_cta && (!wide || half == grp)) {
-                            uint32_t r[32];
-                            const bool full = col0 + 32 <= p.n_cta;       // n_cta is a multiple of 16
-                            if (full) tmem_ld32_sync(t_lane + col0, r);
-                            else tmem_ld16_sync(t_lane + col0, r);
-                            if (grp == 0 && elected && cb == 0 && half == 0) TC_TRACE(8, tr);
+                    for (int i = 0; i < 8; ++i) {                        // 8-column group i: this thread's channel pair of rows r0, r0 + 8
+                        if (cb * 64 + i * 8 < p.n_cta) {                 // n_cta is a multiple of 16
+                            const float4 af = *reinterpret_cast<const float4*>(aff + cb * 64 + i * 8 + cq);   // (s0, s1, b0, b1)
+                            const f32x2 sc = f32x2_make(af.x, af.y), bi = f32x2_make(af.z, af.w);
 #pragma unroll
-                            for (int g = 0; g < 4; ++g) {                 // 8 channels -> one 16-byte chunk
-                                if (g >= 2 && !full) break;
-                                uint32_t pk[4];
-                                float4 af[4];                             // (s0, s1, b0, b1) x 4: independent broadcast loads first
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) af[j] = *reinterpret_cast<const float4*>(aff + col0 + g * 8 + 2 * j);
-#pragma unroll
-                                for (int j = 0; j < 4; ++j)
-                                    pk[j] = MF::template pack_act<RELU6>(ffma2_abc(
-                                        f32x2_make(__uint_as_float(r[g * 8 + 2 * j]), __uint_as_float(r[g * 8 + 2 * j + 1])),
-                                        f32x2_make(af[j].x, af[j].y), f32x2_make(af[j].z, af[j].w)));
-                                *reinterpret_cast<uint4*>(row + (((half * 4 + g) ^ (m & 7)) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+                            for (int h = 0; h < 2; ++h) {
+                                const int r = r0 + 8 * h;
+                                *reinterpret_cast<uint32_t*>(stg + r * 128 + ((i ^ (r & 7)) << 4) + cq * 2) =
+                                    MF::template pack_act<RELU6>(ffma2_abc(f32x2_make(acc[cb][4 * i + 2 * h], acc[cb][4 * i + 2 * h + 1]), sc, bi));
                             }
                         }
                     }
-                    if (cb == cb_last) {                                  // last TMEM read of this item: release the accumulator early
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(smem_u32(&bars->acc_empty[ab]));
-                    }
                     if (p.epi_tma) {
-                        // one elected thread per group, asynchronous, whole 128-byte lines, image borders and channel
-                        // tails clipped by the hardware.  Before anyone may overwrite the other staging buffer its previous
-                        // store must have finished READING shared memory.
+                        // one elected thread, asynchronous, whole 128-byte lines, image borders and channel tails clipped by the
+                        // hardware.  Before anyone may overwrite the other staging buffer its previous store must have finished
+                        // READING shared memory.
                         fence_proxy_async();
-                        if (grp == 0 && elected && cb == 0) TC_TRACE(9, tr);
+                        if (elected && cb == 0) TC_TRACE(9, tr);
                         if (elected) bulk_wait_read0();
                         asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");    // staging tile complete + other buffer free
-                        if (grp == 0 && elected && cb == 0) TC_TRACE(10, tr);
+                        if (elected && cb == 0) TC_TRACE(10, tr);
                         if (elected) {
                             const uint32_t src = smem_u32(stg);
                             const int cc = c.n0 + cb * 64;
@@ -682,19 +613,18 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                                 tma_reduce_add_4d(&tm_o3, src, cc, c.ox0, c.oy0, c.img0);
                             }
                             bulk_commit_group();
-                            if (grp == 0 && cb == 0) TC_TRACE(11, tr);
+                            if (cb == 0) TC_TRACE(11, tr);
                         }
                         continue;
                     }
                     asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");        // staging tile complete
-                    const int et = (wide ? grp * 128 : 0) + q * 32 + lane;   // 0..127 (0..255) over the group's warps
+                    const int et = ew * 32 + lane;                        // 0..255 over the consumer warps
                     const int ch = et & 7;                                // 16-byte chunk within the 64-channel block
                     const int ccol = cb * 64 + ch * 8;                    // accumulator column of that chunk
                     const bool cok = ccol < p.n_cta && c.n0 + ccol + 8 <= p.c_out;
 #pragma unroll
-                    for (int k = 0; k < 8; ++k) {
-                        const int rr = (et >> 3) + (wide ? 32 : 16) * k;  // pixel row of the tile
-                        if (rr >= 128) break;
+                    for (int k = 0; k < 4; ++k) {
+                        const int rr = (et >> 3) + 32 * k;                // pixel row of the tile
                         const int r_ni = rr / (TH * TW), r_ty = (rr / TW) % TH, r_tx = rr % TW;
                         const int pimg = c.img0 + r_ni, poy = c.oy0 + r_ty, pox = c.ox0 + r_tx;
                         if (!(cok && pimg < p.n && poy < p.h_out && pox < p.w_out)) continue;
@@ -736,54 +666,47 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                     }
                 }
             } else {
-                // decode_conv6 folded below the last upsample: dot over this block's (<= 64) output channels, on channel PAIRS:
-                // BN affine as one FFMA2, ReLU folded into the 16-bit rounding (decode_conv5's output IS stored in 16 bits in the
-                // reference), then the head's 16-bit weights times the 16-bit activations on the mixed-precision FMA (exact
-                // products, fp32 accumulation) -- 6 instructions per pair instead of 11
-                const int batches = (p.n_cta + 31) >> 5;
-                float dot_lo = 0.f, dot_hi = 0.f;
-                for (int b = 0; b < batches; ++b) {
-                    uint32_t r[32];
-                    const bool full = b * 32 + 32 <= p.n_cta;
-                    if (full) tmem_ld32_sync(t_lane + b * 32, r);
-                    else tmem_ld16_sync(t_lane + b * 32, r);
+                // decode_conv6 folded below the last upsample: dot over the block's (<= 64) output channels, on channel PAIRS:
+                // BN affine, ReLU folded into the 16-bit rounding (decode_conv5's output IS stored in 16 bits in the reference),
+                // then the head's 16-bit weights times the 16-bit activations (exact products, fp32 accumulation); the four
+                // threads that share a row add their partial dots
+                float dot[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        if (j >= 8 && !full) break;
-                        const int c0 = b * 32 + 2 * j;
+                for (int i = 0; i < 8; ++i) {
+                    const int c0 = i * 8 + cq;
+                    if (i * 8 < p.n_cta) {
                         const float4 af = *reinterpret_cast<const float4*>(s_pw_affine + c0);
-                        const uint32_t h = MF::template pack_act<RELU6>(ffma2_abc(
-                            f32x2_make(__uint_as_float(r[2 * j]), __uint_as_float(r[2 * j + 1])), f32x2_make(af.x, af.y), f32x2_make(af.z, af.w)));
-                        MF::fma2(dot_lo, dot_hi, h, s_head_w2[c0 >> 1]);
+                        const f32x2 sc = f32x2_make(af.x, af.y), bi = f32x2_make(af.z, af.w);
+                        const uint32_t hw = s_head_w2[c0 >> 1];
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const uint32_t hv = MF::template pack_act<RELU6>(ffma2_abc(f32x2_make(acc[0][4 * i + 2 * h], acc[0][4 * i + 2 * h + 1]), sc, bi));
+                            MF::fma2(dot[h][0], dot[h][1], hv, hw);
+                        }
                     }
                 }
-                const float dot = dot_lo + dot_hi;
-                tc_fence_before();                                       // accumulator drained
-                __syncwarp();
-                if (lane == 0) mbar_arrive(smem_u32(&bars->acc_empty[ab]));
-                if (valid) {
-                    const float y = apply_act(fmaf(dot, p.head_scale, p.head_bias), p.head_act);
-                    const uint32_t yy = MF::pack(y, y);
-                    T* ho = reinterpret_cast<T*>(p.head_out) + ((size_t)img * 2 * p.h_out + 2 * oy) * (2 * p.w_out) + 2 * ox;
-                    *reinterpret_cast<uint32_t*>(ho) = yy;
-                    *reinterpret_cast<uint32_t*>(ho + 2 * p.w_out) = yy;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float d = dot[h][0] + dot[h][1];
+                    d += __shfl_xor_sync(0xffffffffu, d, 1);
+                    d += __shfl_xor_sync(0xffffffffu, d, 2);
+                    const int r = r0 + 8 * h;
+                    const int img = c.img0 + r / (TH * TW), oy = c.oy0 + (r / TW) % TH, ox = c.ox0 + r % TW;
+                    if ((lane & 3) == 0 && img < p.n && oy < p.h_out && ox < p.w_out) {
+                        const float y = apply_act(fmaf(d, p.head_scale, p.head_bias), p.head_act);
+                        const uint32_t yy = MF::pack(y, y);
+                        T* ho = reinterpret_cast<T*>(p.head_out) + ((size_t)img * 2 * p.h_out + 2 * oy) * (2 * p.w_out) + 2 * ox;
+                        *reinterpret_cast<uint32_t*>(ho) = yy;
+                        *reinterpret_cast<uint32_t*>(ho + 2 * p.w_out) = yy;
+                    }
                 }
             }
-            if (grp == 0 && elected) { TC_TRACE(7, tr); ++tr; }
-            if (cs) {                                      // every item: next accumulator (or the same one, next phase)
-                if (p.nacc == 2) { ab ^= 1u; if (ab == 0u) pa ^= 1u; } else { pa ^= 1u; }
-            } else if (ngrp == 2) { pa ^= 1u; } else { ab ^= 1u; if (ab == 0u) pa ^= 1u; }
+            if (elected) TC_TRACE(7, tr);
         }
-        if (p.epi_tma && elected) bulk_wait_all();                       // all tensor stores of this group have landed
+        if (p.epi_tma && elected) bulk_wait_all();                       // all tensor stores have landed
     }
 
-    tc_fence_before();
     if constexpr (CLM != 0) cluster_sync_all();    // nobody leaves while a peer may still copy into / signal this CTA
-    else __syncthreads();
-    if (warp == TC_WARP_MMA) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-    }
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -816,17 +739,13 @@ struct BlockTcPlan {
     std::string name;
 };
 
-// experiment knobs (environment, read when a plan is built): FD_TC_MAX_NCTA=<n>, FD_TC_NO_COLSPLIT=1
+// experiment knobs (environment, read when a plan is built): FD_TC_MAX_NCTA=<n>, FD_TC_CLUSTER=1|2|4, FD_TC_CLUSTER_MULTIWAVE=1
 static void plan_env_knobs(BlockPlanIn& q) {
     const char* a = getenv("FD_TC_MAX_NCTA");
-    const char* b = getenv("FD_TC_NO_COLSPLIT");
-    const char* c = getenv("FD_TC_NO_WIDE");
     const char* d = getenv("FD_TC_CLUSTER");          // 1 = never, 2 / 4 = force that cluster size where the block admits it
     if (d && *d) q.cluster = atoi(d);
     { const char* m = getenv("FD_TC_CLUSTER_MULTIWAVE"); q.cluster_multiwave = (m && *m == '1') ? 1 : 0; }
-    q.no_wide = (c && *c == '1') ? 1 : 0;
     q.max_n_cta = a ? atoi(a) : 0;
-    q.no_colsplit = (b && *b == '1') ? 1 : 0;
 }
 
 static int pick_tile(const StageGeom& g) {
@@ -933,7 +852,7 @@ BlockPlanOut block_tc_debug_plan(int ksize, int stride, int h_out, int w_out, in
     q.ksize = ksize; q.stride = stride; q.tile = pick_tile(g); q.c_in = c_in; q.c_out = c_out; q.head = head;
     const int NI = q.tile ? 2 : 1, TW = q.tile ? 8 : 16;
     q.n_tiles = ((w_out + TW - 1) / TW) * ((h_out + 7) / 8) * ((n + NI - 1) / NI);
-    q.barrier_bytes = (int)sizeof(TcBarriers); q.n_sms = 148;
+    q.barrier_bytes = (int)sizeof(TcBarriers); q.n_sms = 132;
     q.cluster = 0;
     { const char* e = getenv("FD_TC_DW_TEAMS"); q.even_rings = (e && *e == '1') ? 0 : ((e && *e == '2') ? 1 : 2); }
     if (q.even_rings == 2 && ksize == 5 && (c_in + TC_KBLK - 1) / TC_KBLK <= 2) q.even_rings = 1;
@@ -979,7 +898,7 @@ __global__ void pack_dwp_kernel(const float* __restrict__ w, const float* __rest
 __global__ void pack_affine_kernel(const float* __restrict__ scale, const float* __restrict__ bias, float2* __restrict__ dst,
                                    int n_src, int n_dst, float post) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    // per channel PAIR (2j, 2j+1): (scale, scale, bias, bias), so that one 16-byte load feeds an FFMA2
+    // per channel PAIR (2j, 2j+1): (scale, scale, bias, bias), so that one 16-byte load feeds the pair's affine
     if (i < n_dst) {
         const int pair = i >> 1, odd = i & 1;
         float* d = reinterpret_cast<float*>(dst) + pair * 4;
@@ -1038,25 +957,23 @@ int block_tc_prepare(int dtype, const BlockArgs& a, const float* head_w, float h
     pin.head = p.head; pin.barrier_bytes = (int)sizeof(TcBarriers); pin.n_sms = opts.n_sms;
     pin.cluster = (opts.cluster && !bp->halfk) ? 0 : 1;
     { const char* e = getenv("FD_TC_DW_TEAMS"); pin.even_rings = (e && *e == '1') ? 0 : ((e && *e == '2') ? 1 : 2); }   // 1 = never, 2 = wherever even rings fit
-    if (pin.even_rings == 2 && g.ksize == 5 && (g.c_in + TC_KBLK - 1) / TC_KBLK <= 2) pin.even_rings = 1;   // decode_conv4: in4/a2 + teams 59.4 -> 57.5 us
+    if (pin.even_rings == 2 && g.ksize == 5 && (g.c_in + TC_KBLK - 1) / TC_KBLK <= 2) pin.even_rings = 1;   // 5x5 blocks of <= 2 K-blocks
     plan_env_knobs(pin);
     if (bp->halfk) pin.cluster = 1;
     const BlockPlanOut po = plan_block(pin);
     if (!po.ok) { delete bp; return fail(FD_ERR_UNSUPPORTED, "fused block does not fit shared memory"); }
     const int splits = po.splits;
-    p.n_cta = po.n_cta; p.splits = po.splits; p.items = po.items; p.nacc = po.nacc; p.tmem_cols = po.tmem_cols;
-    p.epi_colsplit = po.epi_colsplit; p.epi_wide = po.epi_wide;
+    p.n_cta = po.n_cta; p.splits = po.splits; p.items = po.items;
     p.in_stage_bytes = po.in_stage_bytes; p.dwp_bytes = po.dwp_bytes; p.in_stage_stride = po.in_stage_stride; p.cpad_all = po.cpad_all;
-    p.s_a = po.s_a; p.n_stg = po.n_stg; p.epi_groups = po.epi_groups; p.s_in = po.s_in; p.s_b = po.s_b; p.bn = po.bn; p.nb = po.nb;
+    p.s_a = po.s_a; p.n_stg = po.n_stg; p.s_in = po.s_in; p.s_b = po.s_b; p.bn = po.bn; p.nb = po.nb;
     p.b_resident = po.b_resident; p.b_stage_bytes = po.b_stage_bytes;
     p.cs = po.cs; bp->tiles = n_tiles;
     // Weight-multicast clusters (mode 2): wmc consecutive tiles with the same output-channel split stream ONE copy of the weights
-    // out of the L2 -- the small-map blocks move 110-125 MB through the L2 -> SM fabric per launch, more than half of it the same
-    // weight blocks fetched again by every CTA (ncu l1tex__m_xbar2l1tex_read_bytes, profiles/r02_v1_kernels.csv).
+    // out of the L2 instead of every CTA fetching the same weight blocks again.
     { const char* e = getenv("FD_TC_EPI_HIGH"); p.epi_high = (e && *e) ? atoi(e) : 0; }
-    // Two depthwise teams (see the kernel): measured -3 % on the single-K-block blocks (conv1 57.2 -> 55.4 us, decode_conv5
-    // 88.1 -> 85.4); where the even ring depths it needs cost the plan a staging tile or a weight stage it loses (conv3 +9 %), so:
-    // automatic only for one-K-block blocks whose unconstrained plan already has even rings; FD_TC_DW_TEAMS=2 forces even rings.
+    // Two depthwise teams (see the kernel) need even ring depths, which can cost the plan a staging tile or a weight stage, so
+    // they are automatic only for one-K-block blocks whose unconstrained plan already has even rings; FD_TC_DW_TEAMS=2 forces
+    // even rings.
     p.dw_teams = po.dw_teams;
     p.wmc = 1;
     {
@@ -1153,9 +1070,9 @@ int block_tc_prepare(int dtype, const BlockArgs& a, const float* head_w, float h
     if (p.cs > 1) snprintf(clbuf, sizeof(clbuf), ",cl%d", p.cs);
     else if (p.wmc > 1) snprintf(clbuf, sizeof(clbuf), ",wmc%d", p.wmc);
     if (p.dw_teams == 2) strncat(clbuf, ",t2", sizeof(clbuf) - strlen(clbuf) - 1);
-    snprintf(buf, sizeof(buf), "block_tc<k%d,s%d,%s%s%s>%s%s%s[n%dx%d,bn%d%s,kb%d,in%d,a%d,b%d,e%dx%d%s]", g.ksize, g.stride, bp->tile ? "2x8x8" : "1x8x16", bp->halfk ? ",k32" : "", clbuf,
+    snprintf(buf, sizeof(buf), "block_tc<k%d,s%d,%s%s%s>%s%s%s[n%dx%d,bn%d%s,kb%d,in%d,a%d,b%d,e%d]", g.ksize, g.stride, bp->tile ? "2x8x8" : "1x8x16", bp->halfk ? ",k32" : "", clbuf,
              g.upsample ? "+up2x" : "", a.skip ? (p.epi_red ? "+skip(red)" : "+skip") : "", p.head ? "+head" : (p.epi_tma ? "+tmast" : ""), p.n_cta, p.splits, p.bn,
-             p.b_resident ? "r" : "", p.kblocks, p.s_in, p.s_a, p.s_b, p.epi_groups, p.head ? 0 : p.n_stg / p.epi_groups, p.epi_colsplit ? "c" : (p.epi_wide ? "w" : ""));
+             p.b_resident ? "r" : "", p.kblocks, p.s_in, p.s_a, p.s_b, p.head ? 0 : p.n_stg);
     bp->name = buf;
     *out = bp;
     return FD_OK;

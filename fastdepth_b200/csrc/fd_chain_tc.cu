@@ -6,18 +6,18 @@
 //   * The CTA pair splits the image by ROWS (CTA 0: rows [0, rows0), CTA 1: the rest): each CTA keeps its rows plus one halo row
 //     above and below for all channels, as <= 8 K-blocks of [9 rows][15 px][64 ch] (pixel pitch 15: column 14 is a zero column
 //     that serves as the right padding of its row and the left padding of the next one), 128 B per pixel, 16-byte chunks
-//     XOR-swizzled with the pixel slot index -- the SWIZZLE_128B pattern TMA writes and tcgen05 reads.
-//   * Depthwise (16 warps, lane = channel pair, 4x4 pixels per warp, FFMA2 like the block kernel): reads a K-block's pixels,
+//     XOR-swizzled with the pixel slot index -- the SWIZZLE_128B pattern TMA writes and wgmma reads.
+//   * Depthwise (16 warps, lane = channel pair, 2 columns x 7 rows per warp): reads a K-block's pixels,
 //     and -- after the eight warps working on that K-block have all finished reading -- writes the 128 result rows IN PLACE over
 //     the block in the K-major SWIZZLE_128B operand layout.  The block is then the A operand of that K-block; there is no
 //     separate A ring (the shared memory holds 136 KB of activations + a 64 KB weight ring).
-//   * Pointwise: tcgen05.mma.cta_group::2, M = 256 over the pair (each CTA its own 128 pixel slots), N <= 256 per instruction,
-//     each CTA supplying HALF of every weight tile through its own TMA (completion posted on the leader's mbarrier), fp32
-//     accumulators for all <= 512 output channels in both CTAs' TMEM.  Only the leader CTA issues MMAs; tcgen05.commit
-//     multicasts stage-free / accumulator-ready to both CTAs.
-//   * Epilogue (the same 16 warps): TMEM -> BN affine (FFMA2) + ReLU6 -> 16-bit -> the NEXT layer's activation blocks in shared
-//     memory; the boundary row also goes into the peer CTA's halo row (st.shared::cluster), then one remote mbarrier arrive per
-//     warp tells the peer its halo is complete.  The last layer stores to global memory instead.
+//   * Pointwise (the same 16 warps = four warpgroups): each CTA runs wgmma on its own 128 pixel slots with whole weight tiles
+//     [128 output channels][64 K] streamed by its own TMA.  The output channels go in passes of 128: warpgroup (rh, ch) owns
+//     rows [64 rh, 64 rh + 64) and columns [64 ch, 64 ch + 64) of the pass, accumulates over every K-block in registers
+//     (wgmma.m64n64k16), applies BN + act and keeps the 16-bit result in registers -- the activation blocks are still the
+//     A operand of the later passes.  After the last pass all results go into the NEXT layer's activation blocks in shared
+//     memory; the boundary row also goes into the peer CTA's halo row (st.shared::cluster), then one remote mbarrier arrive
+//     tells the peer its halo is complete.  The last layer stores to global memory instead.
 //
 // Layer boundaries therefore cost a named barrier + one DSMEM hand-shake instead of a kernel boundary; weights for the next
 // K-blocks / layer stream through the 4-deep ring while the epilogue runs.
@@ -35,8 +35,9 @@
 namespace fd {
 
 constexpr int CH_WORKERS = 16;                       // warps 0..15: depthwise + epilogue
-constexpr int CH_WARP_TMA = 16, CH_WARP_MMA = 17;
-constexpr int CH_THREADS = 18 * 32;
+constexpr int CH_WARP_TMA = 16;
+constexpr int CH_THREADS = 17 * 32;
+constexpr int CH_MAX_PASS = 4;                       // output channels per layer <= CH_MAX_PASS x 128
 constexpr int CH_MAX_LAYERS = 8, CH_MAX_KB = 8;
 constexpr int CH_PITCH = 15, CH_ROWS = 9;            // pixel slots: slot(r, c) = r * 15 + c, r in [0, 9), c in [0, 15)
 constexpr int CH_BLK = 136 * 128;                    // 135 slots + 1 spare zero slot; 17 x 1024 B keeps every block 1 KB aligned
@@ -52,22 +53,22 @@ constexpr int CH_OFF_BAR = CH_OFF_AFF + 2 * CH_AFF_BYTES;
 
 struct ChainBarriers {
     uint64_t in_full[CH_MAX_KB];        // layer-0 input block landed (TMA tx), once per image
-    uint64_t a_full[CH_MAX_KB];         // LEADER's copy is the live one: 16 arrivals (8 depthwise warps of each CTA), once per layer
-    uint64_t b_full[CH_SB];             // LEADER's copy: both CTAs' weight halves landed (tx)
-    uint64_t b_empty[CH_SB];            // tcgen05.commit multicast: stage consumed
+    uint64_t a_full[CH_MAX_KB];         // the 8 depthwise warps of the K-block's group have written its operand tile, once per layer
+    uint64_t b_full[CH_SB];             // weight tile landed (tx)
+    uint64_t b_empty[CH_SB];            // all four warpgroups are done reading the stage
     uint64_t dwp_full[CH_SD], dwp_empty[CH_SD];
     uint64_t aff_full[2], aff_empty[2];
-    uint64_t acc_full;                  // tcgen05.commit multicast: all MMAs of the layer done
+    uint64_t mma_done;                  // one remote arrival: the peer's warpgroups have finished reading their operand tiles, so
+                                        // its halo rows (which the in-place tiles cover) may be overwritten
     uint64_t halo_full;                 // one remote arrival (cluster-scope release): the peer has written my halo row of the next layer
     uint64_t act_free;                  // the last layer's output has left the activation blocks (TMA stores have read them)
-    uint32_t tmem_base, pad;
 };
 constexpr int CH_SMEM_BYTES = CH_OFF_BAR + (int)sizeof(ChainBarriers) + 1024;     // + alignment slack
 
 struct ChainLayer {
     int c_in, c_out;
     int kblocks;           // ceil(c_in / 64)
-    int nh;                // MMA column groups of <= 256: ceil(n_pad / 256)
+    int np;                // passes of 128 output channels: ceil(n_pad / 128)
     int n_pad;             // c_out rounded up to 32 (accumulator columns in use)
     int aff_bytes;         // n_pad * 8
     const void* dwp;       // [kblocks] x CH_DWP bytes
@@ -95,27 +96,8 @@ struct ChainMaps {
                                        // SWIZZLE_128B; column 14 and channels >= c_out are clipped by the hardware
 };
 
-// ---- 2-CTA PTX (cluster helpers: fd_tc_common.cuh) -------------------------------------------------------
-// TMA tile load issued by either CTA of the pair, completion bytes posted on the LEADER's mbarrier
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(dst), "l"(map), "r"(leader_bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma2_f16_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tmov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\tsetp.ne.b32 p, %5, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %4, p;\n\t}" ::"r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc),
-        "r"(acc) : "memory");
-}
-__device__ __forceinline__ void umma2_commit_mc(uint32_t bar) {      // arrive on the barrier at this offset in BOTH CTAs
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"((uint16_t)3) : "memory");
+__device__ __forceinline__ void st_cluster_u32(uint32_t cluster_addr, uint32_t v) {
+    asm volatile("st.shared::cluster.b32 [%0], %1;" ::"r"(cluster_addr), "r"(v) : "memory");
 }
 
 #define CH_TRACE(row, idx)                                                                                \
@@ -139,11 +121,11 @@ chain_tc_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ 
     const int row_first = rank == 0 ? 0 : p.rows0;              // image row of local row 0
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < CH_MAX_KB; ++i) { mbar_init(smem_u32(&bars->in_full[i]), 1); mbar_init(smem_u32(&bars->a_full[i]), CH_WORKERS); }
-        for (int i = 0; i < CH_SB; ++i) { mbar_init(smem_u32(&bars->b_full[i]), 1); mbar_init(smem_u32(&bars->b_empty[i]), 1); }
+        for (int i = 0; i < CH_MAX_KB; ++i) { mbar_init(smem_u32(&bars->in_full[i]), 1); mbar_init(smem_u32(&bars->a_full[i]), CH_WORKERS / 2); }
+        for (int i = 0; i < CH_SB; ++i) { mbar_init(smem_u32(&bars->b_full[i]), 1); mbar_init(smem_u32(&bars->b_empty[i]), CH_WORKERS / 4); }
         for (int i = 0; i < CH_SD; ++i) { mbar_init(smem_u32(&bars->dwp_full[i]), 1); mbar_init(smem_u32(&bars->dwp_empty[i]), CH_WORKERS / 2); }
         for (int i = 0; i < 2; ++i) { mbar_init(smem_u32(&bars->aff_full[i]), 1); mbar_init(smem_u32(&bars->aff_empty[i]), CH_WORKERS); }
-        mbar_init(smem_u32(&bars->acc_full), 1);
+        mbar_init(smem_u32(&bars->mma_done), 1);
         mbar_init(smem_u32(&bars->halo_full), 1);
         mbar_init(smem_u32(&bars->act_free), 1);
         fence_barrier_init();
@@ -151,7 +133,6 @@ chain_tc_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ 
     // every activation slot starts as finite zeros (padding, channels a narrower layer never writes)
     for (int i = threadIdx.x; i < (CH_OFF_B) / 16; i += CH_THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0u, 0u, 0u, 0u);
     fence_proxy_async();
-    if (warp == CH_WARP_MMA) tmem_alloc_2cta(smem_u32(&bars->tmem_base), 512u);
     if (warp == CH_WARP_TMA && lane == 0) {
         tma_prefetch_desc(&maps.in);
         tma_prefetch_desc(&maps.out[rank]);
@@ -159,29 +140,23 @@ chain_tc_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ 
     }
     pdl_launch_dependents();
     pdl_wait_prior_grid();                         // everything below reads what the previous kernel wrote
-    tc_fence_before();
     cluster_sync_all();                            // barriers initialised + smem zeroed in BOTH CTAs before any remote access
-    tc_fence_after();
-    const uint32_t tmem_base = bars->tmem_base;
 
     if (warp == CH_WARP_TMA) {
         // =========================== producers (single threads) ===========================
         if (lane == 0) {
-            // pointwise weights: this CTA's half (rows rank * N/2 ...) of every [N <= 256][64] tile, all layers, all images
-            const uint32_t leader_b_full0 = mapa_u32(smem_u32(&bars->b_full[0]), 0);
+            // pointwise weights: [128 output channels][64 K] tiles in the order the passes consume them, all layers, all images
             uint32_t seq = 0;
             for (int img = cluster_id; img < p.n_img; img += n_clusters)
                 for (int l = 0; l < p.n_layers; ++l) {
                     const ChainLayer& L = p.L[l];
-                    for (int kb = 0; kb < L.kblocks; ++kb)
-                        for (int nh = 0; nh < L.nh; ++nh, ++seq) {
+                    for (int ps = 0; ps < L.np; ++ps)
+                        for (int kb = 0; kb < L.kblocks; ++kb, ++seq) {
                             const uint32_t s = seq & (CH_SB - 1), ph = (seq / CH_SB) & 1u;
                             mbar_wait_sleep(smem_u32(&bars->b_empty[s]), ph ^ 1u, (uint32_t)p.sleep_ns);
-                            if (kb == 0 && nh == 0 && img == cluster_id) CH_TRACE(10, l);
-                            const int n_ins = min(256, L.n_pad - nh * 256);
-                            if (rank == 0) mbar_expect_tx(smem_u32(&bars->b_full[s]), 2u * CH_B_STAGE);
-                            tma_load_2d_2sm(smem_base + CH_OFF_B + s * CH_B_STAGE, &maps.w[l], leader_b_full0 + 8u * s, kb * 64,
-                                            nh * 256 + (int)rank * (n_ins >> 1));
+                            if (kb == 0 && ps == 0 && img == cluster_id) CH_TRACE(10, l);
+                            mbar_expect_tx(smem_u32(&bars->b_full[s]), (uint32_t)CH_B_STAGE);
+                            tma_load_2d(smem_base + CH_OFF_B + s * CH_B_STAGE, &maps.w[l], smem_u32(&bars->b_full[s]), kb * 64, ps * 128);
                         }
                 }
         } else if (lane == 1) {
@@ -216,48 +191,13 @@ chain_tc_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ 
                 }
             }
         }
-    } else if (warp == CH_WARP_MMA) {
-        // =========================== MMA issuer (leader CTA, one thread) ===========================
-        if (rank == 0 && lane == 0) {
-            const uint32_t idesc_base = (1u << 4) | (MF::kUmmaFormat << 7) | (MF::kUmmaFormat << 10) | ((256u >> 4) << 24);
-            const uint32_t a_lo0 = sw128_desc_lo(smem_base + CH_OFF_ACT), b_lo0 = sw128_desc_lo(smem_base + CH_OFF_B);
-            uint32_t seq = 0, a_par = 0;
-            for (int img = cluster_id; img < p.n_img; img += n_clusters)
-                for (int l = 0; l < p.n_layers; ++l) {
-                    const ChainLayer& L = p.L[l];
-                    for (int kb = 0; kb < L.kblocks; ++kb) {
-                        mbar_wait(smem_u32(&bars->a_full[kb]), (a_par >> kb) & 1u);      // CTA-scope acquire: a cluster-scope one costs a CCTL.IVALL per probe
-                        a_par ^= 1u << kb;
-                        tc_fence_after();
-                        if (kb == 0 && img == cluster_id) CH_TRACE(7, l);
-                        const uint32_t a_lo = a_lo0 + (uint32_t)kb * (CH_BLK >> 4);
-                        for (int nh = 0; nh < L.nh; ++nh, ++seq) {
-                            const uint32_t s = seq & (CH_SB - 1), ph = (seq / CH_SB) & 1u;
-                            mbar_wait(smem_u32(&bars->b_full[s]), ph);
-                            tc_fence_after();
-                            if (kb == 0 && nh == 0 && img == cluster_id) CH_TRACE(11, l);
-                            const int n_ins = min(256, L.n_pad - nh * 256);
-                            const uint32_t idesc = idesc_base | ((uint32_t)(n_ins >> 3) << 17);
-                            const uint32_t b_lo = b_lo0 + s * (CH_B_STAGE >> 4);
-                            const uint32_t dcol = tmem_base + (uint32_t)(nh * 256);
-                            umma2_f16_lohi(dcol, a_lo, b_lo, kSw128DescHi, idesc, kb > 0 ? 1u : 0u);
-                            umma2_f16_lohi(dcol, a_lo + 2, b_lo + 2, kSw128DescHi, idesc, 1u);
-                            umma2_f16_lohi(dcol, a_lo + 4, b_lo + 4, kSw128DescHi, idesc, 1u);
-                            umma2_f16_lohi(dcol, a_lo + 6, b_lo + 6, kSw128DescHi, idesc, 1u);
-                            umma2_commit_mc(smem_u32(&bars->b_empty[s]));
-                        }
-                    }
-                    umma2_commit_mc(smem_u32(&bars->acc_full));
-                    if (img == cluster_id) CH_TRACE(8, l);
-                }
-        }
     } else {
         // =========================== workers: depthwise, then epilogue, per layer ===========================
         const int grp = warp >> 3, wi = warp & 7;
         // Depthwise mapping: a CTA owns at most 7 rows x 14 columns, so warp wi < 7 computes the two columns 2 wi, 2 wi + 1 of
         // all seven rows (14 outputs from a 9 x 4 input patch; every computed pixel can be a real one) and the eighth warp of the
-        // group only takes part in the hand-shakes.  (A 4x4-blocks-of-an-8x16-tile mapping spends 23 % of its FMAs on slots
-        // that are never pixels and was measured at 4 800 cycles per K-block pair.)
+        // group only takes part in the hand-shakes.  (A 4x4-blocks-of-an-8x16-tile mapping would spend 23 % of its FMAs on
+        // slots that are never pixels.)
         const bool dw_active = wi < 7;
         const int tx0 = 2 * (dw_active ? wi : 0);
         const int s0 = tx0 - 1;                                             // slot of the patch's top-left pixel (-1: the spare zero slot)
@@ -272,19 +212,27 @@ chain_tc_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ 
         // zero list: thread t < n_zero * 8 re-zeroes 16-byte chunk (t & 7) of slot zero_slots[t >> 3] in every K-block
         const int nzc = p.n_zero[rank] * 8;
         const uint32_t z_off = (int)threadIdx.x < nzc ? (uint32_t)p.zero_slots[rank][threadIdx.x >> 3] * 128u + ((uint32_t)threadIdx.x & 7u) * 16u : 0u;
-        // epilogue role: TMEM lane quarter q = warp % 4, 32-column blocks cq, cq + 4, ...; thread = pixel slot m
-        const int q = warp & 3, cq = warp >> 2;
-        const int m = q * 32 + lane, e_ty = m >> 4, e_tx = m & 15;
-        const bool e_valid = e_ty < rows_local && e_tx < p.w;
-        const int e_slot = (e_ty + 1) * CH_PITCH + e_tx;                    // where this pixel lives in the next layer's input blocks
-        // boundary rows also go to the peer: CTA 0's last row is CTA 1's top halo (its buffer row 0), CTA 1's first row is
-        // CTA 0's bottom halo (buffer row rows0 + 1)
-        const bool e_halo = e_valid && (rank == 0 ? e_ty == rows_local - 1 : e_ty == 0);
-        const int e_halo_slot = (rank == 0 ? 0 : (p.rows0 + 1) * CH_PITCH) + e_tx;
+        // pointwise role: warpgroup (rh, ch) = operand rows [64 rh, +64) x pass columns [64 ch, +64); a thread holds rows
+        // m and m + 8 (m = 64 rh + 16 (warp % 4) + lane / 4) and the channel pair cp of every 8-column group
+        const int rh = (warp >> 2) & 1, ch = warp >> 3, cp = (lane & 3) * 2;
+        const bool wg_leader = (warp & 3) == 0 && lane == 0;
+        int e_slot[2], e_halo_slot[2], e_last_slot[2];
+        bool e_valid[2], e_halo[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int m = rh * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h, e_ty = m >> 4, e_tx = m & 15;
+            e_valid[h] = e_ty < rows_local && e_tx < p.w;
+            e_slot[h] = (e_ty + 1) * CH_PITCH + e_tx;                       // where this pixel lives in the next layer's input blocks
+            e_last_slot[h] = e_ty * CH_PITCH + e_tx;                        // the last layer's staging slot
+            // boundary rows also go to the peer: CTA 0's last row is CTA 1's top halo (its buffer row 0), CTA 1's first row is
+            // CTA 0's bottom halo (buffer row rows0 + 1)
+            e_halo[h] = e_valid[h] && (rank == 0 ? e_ty == rows_local - 1 : e_ty == 0);
+            e_halo_slot[h] = (rank == 0 ? 0 : (p.rows0 + 1) * CH_PITCH) + e_tx;
+        }
         const uint32_t peer_act = mapa_u32(smem_base + CH_OFF_ACT, rank ^ 1u);
-        const uint32_t leader_a_full0 = mapa_u32(smem_u32(&bars->a_full[0]), 0);
         const uint32_t peer_halo_full = mapa_u32(smem_u32(&bars->halo_full), rank ^ 1u);
-        uint32_t dseq_base = 0, lseq = 0, halo_seq = 0, it = 0;
+        const uint32_t peer_mma_done = mapa_u32(smem_u32(&bars->mma_done), rank ^ 1u);
+        uint32_t dseq_base = 0, lseq = 0, halo_seq = 0, it = 0, bseq = 0, a_par = 0;
         for (int img = cluster_id; img < p.n_img; img += n_clusters, ++it) {
             for (int l = 0; l < p.n_layers; ++l, ++lseq) {
                 const ChainLayer& L = p.L[l];
@@ -302,45 +250,6 @@ chain_tc_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ 
                     const f32x2 bi = *reinterpret_cast<const f32x2*>(prm + 9 * 128 + 256 + lane * 8);
                     const uint8_t* in0 = blk + s0 * 128;
                     uint32_t o[7][2];
-#ifdef FD_CHAIN_DW_FHFMA       // build-time A/B: measured 83.5 us against 79.1 us for the FFMA2 form below (the MMA stream, which shares
-                              // the schedulers with the workers, finishes later under the denser FHFMA stream)
-                    // 16-bit x 16-bit + fp32 on FHFMA (0.84 / clk / scheduler, no widening): with four worker warps per scheduler
-                    // the FMA pipe is the limit, where 252 FHFMA beat 126 FFMA2 + 90 HADD2.F32 (both pairs of two-cycle
-                    // instructions); bit-identical either way (exact products, same accumulation order)
-                    if (dw_active) {
-                        uint32_t wv[9];
-#pragma unroll
-                        for (int i = 0; i < 9; ++i) wv[i] = *reinterpret_cast<const uint32_t*>(prm + i * 128 + lane * 4);
-                        float acc[7][2][2];
-#pragma unroll
-                        for (int a = 0; a < 7; ++a)
-#pragma unroll
-                            for (int b = 0; b < 2; ++b) acc[a][b][0] = acc[a][b][1] = 0.f;
-#pragma unroll
-                        for (int iy = 0; iy < 9; ++iy) {
-                            uint32_t row[4];
-#pragma unroll
-                            for (int ix = 0; ix < 4; ++ix) {
-                                const int k = iy * CH_PITCH + ix;
-                                row[ix] = *reinterpret_cast<const uint32_t*>(in0 + k * 128 + rd_off[k & 7]);
-                            }
-#pragma unroll
-                            for (int oy = 0; oy < 7; ++oy) {
-                                const int ky = iy - oy;
-                                if (ky < 0 || ky >= 3) continue;
-#pragma unroll
-                                for (int ox = 0; ox < 2; ++ox)
-#pragma unroll
-                                    for (int kx = 0; kx < 3; ++kx) MF::fma2(acc[oy][ox][0], acc[oy][ox][1], row[ox + kx], wv[ky * 3 + kx]);
-                            }
-                        }
-#pragma unroll
-                        for (int oy = 0; oy < 7; ++oy)
-#pragma unroll
-                            for (int ox = 0; ox < 2; ++ox)
-                                o[oy][ox] = MF::template pack_act<RELU6>(ffma2_abc(f32x2_make(acc[oy][ox][0], acc[oy][ox][1]), sc, bi));
-                    }
-#else
                     if (dw_active) {
                         f32x2 acc[7][2];
 #pragma unroll
@@ -373,7 +282,6 @@ chain_tc_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ 
 #pragma unroll
                             for (int ox = 0; ox < 2; ++ox) o[oy][ox] = MF::template pack_act<RELU6>(ffma2_abc(acc[oy][ox], sc, bi));
                     }
-#endif
                     __syncwarp();
                     if (tr0 && kb == 0) CH_TRACE(1, l);
                     if (lane == 0) mbar_arrive(smem_u32(&bars->dwp_empty[ds]));
@@ -388,52 +296,86 @@ chain_tc_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ 
                     }
                     fence_proxy_async();                       // generic-proxy writes -> visible to the tensor cores (async proxy)
                     __syncwarp();
-                    if (lane == 0) mbar_arrive_remote_cta_scope(leader_a_full0 + 8u * (uint32_t)kb);
+                    if (lane == 0) mbar_arrive(smem_u32(&bars->a_full[kb]));
                 }
                 dseq_base += (uint32_t)L.kblocks;
                 if (tr0) CH_TRACE(2, l);
                 if (tr8) CH_TRACE(9, l);
 
-                // ---------------- epilogue: accumulator -> next layer's activations (or global memory) ----------------
-                mbar_wait_sleep(smem_u32(&bars->acc_full), lseq & 1u, (uint32_t)p.sleep_ns);
-                tc_fence_after();
-                if (tr0) CH_TRACE(3, l);
+                // ---------------- pointwise: passes of 128 output channels over every K-block ----------------
                 const uint32_t as = lseq & 1u;
                 mbar_wait(smem_u32(&bars->aff_full[as]), (lseq >> 1) & 1u);
                 const float2* aff = reinterpret_cast<const float2*>(smem + CH_OFF_AFF + as * CH_AFF_BYTES);
-                const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-                const int ncb = L.n_pad >> 5;
+                uint32_t pk[CH_MAX_PASS][16];                              // [pass][8 h + i]: 16-bit results, channel pair of group i
+#pragma unroll
+                for (int ps = 0; ps < CH_MAX_PASS; ++ps) {
+                    if (ps >= L.np) break;
+                    const int col0 = ps * 128 + ch * 64;                  // first output channel of this warpgroup's block
+                    const bool act = col0 < L.n_pad;
+                    float acc[32];
+#pragma unroll
+                    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+                    for (int kb = 0; kb < L.kblocks; ++kb, ++bseq) {
+                        const uint32_t s = bseq & (CH_SB - 1), ph = (bseq / CH_SB) & 1u;
+                        mbar_wait(smem_u32(&bars->a_full[kb]), (a_par >> kb) & 1u);   // (a no-op after the first pass)
+                        mbar_wait(smem_u32(&bars->b_full[s]), ph);
+                        if (tr0 && kb == 0 && ps == 0) CH_TRACE(7, l);
+                        if (act) {
+                            const uint32_t a_lo = sw128_desc_lo(smem_base + CH_OFF_ACT + (uint32_t)kb * CH_BLK + (uint32_t)rh * 8192u);
+                            const uint32_t b_lo = sw128_desc_lo(smem_base + CH_OFF_B + s * CH_B_STAGE + (uint32_t)ch * 8192u);
+                            wgmma_fence();
+#pragma unroll
+                            for (int k4 = 0; k4 < 4; ++k4)                // +32 B (16 elements) per K step
+                                wgmma_n64<T>(acc, sw128_desc(a_lo + 2u * k4), sw128_desc(b_lo + 2u * k4), (kb > 0 || k4 > 0) ? 1u : 0u);
+                            wgmma_commit();
+                            wgmma_wait0();
+                        }
+                        if (wg_leader) mbar_arrive(smem_u32(&bars->b_empty[s]));
+                    }
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const int c = col0 + i * 8 + cp;
+                        const bool ok = act && col0 + i * 8 < L.n_pad;
+                        const float4 af = ok ? *reinterpret_cast<const float4*>(aff + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+                            pk[ps][8 * h + i] = MF::template pack_act<RELU6>(ffma2_abc(f32x2_make(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]),
+                                                                                        f32x2_make(af.x, af.y), f32x2_make(af.z, af.w)));
+                    }
+                }
+                for (int kb = 0; kb < L.kblocks; ++kb) a_par ^= 1u << kb;
+                if (tr0) CH_TRACE(8, l);
+                // every warpgroup has finished reading the operand tiles: the activation blocks may be overwritten
+                asm volatile("bar.sync %0, %1;" ::"r"(3), "r"(CH_WORKERS * 32) : "memory");
+                if (!last) {                      // ... and so has the peer, before this CTA writes into the peer's halo rows
+                    if (threadIdx.x == 0) mbar_arrive_cluster(peer_mma_done);
+                    mbar_wait_cluster(smem_u32(&bars->mma_done), halo_seq & 1u, 0u);
+                }
+                if (tr0) CH_TRACE(3, l);
                 // the last layer's tile is staged in the (now dead) activation blocks from slot 0 on -- a 1 KB-aligned TMA source --
                 // and leaves through tensor stores; every other layer writes the next layer's input rows 1.. and the peer's halo
-                const int w_slot = last ? e_ty * CH_PITCH + e_tx : e_slot;
-                for (int cb = cq; cb < ncb; cb += 4) {
-                    uint32_t r[32];
-                    tmem_ld32_sync(t_lane + (uint32_t)(cb * 32), r);
-                    uint32_t pk[16];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float4 af = *reinterpret_cast<const float4*>(aff + cb * 32 + 2 * j);
-                        pk[j] = MF::template pack_act<RELU6>(ffma2_abc(f32x2_make(__uint_as_float(r[2 * j]), __uint_as_float(r[2 * j + 1])),
-                                                                        f32x2_make(af.x, af.y), f32x2_make(af.z, af.w)));
-                    }
-                    const uint32_t boff = (uint32_t)(cb >> 1) * CH_BLK, c4 = (uint32_t)(cb & 1) * 4u;
-                    if (e_valid) {
-                        uint8_t* dst = smem + CH_OFF_ACT + boff + w_slot * 128;
+                for (int ps = 0; ps < CH_MAX_PASS; ++ps) {
+                    if (ps >= L.np) break;
+                    const int col0 = ps * 128 + ch * 64;
+                    if (col0 >= L.n_pad) continue;
+                    const uint32_t boff = (uint32_t)(col0 >> 6) * CH_BLK;
 #pragma unroll
-                        for (int g = 0; g < 4; ++g)
-                            *reinterpret_cast<uint4*>(dst + (((c4 + g) ^ ((uint32_t)w_slot & 7u)) << 4)) =
-                                make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-                    }
-                    if (e_halo && !last) {
-                        const uint32_t dst = peer_act + boff + (uint32_t)e_halo_slot * 128u;
+                    for (int h = 0; h < 2; ++h) {
+                        const int w_slot = last ? e_last_slot[h] : e_slot[h];
 #pragma unroll
-                        for (int g = 0; g < 4; ++g)
-                            st_cluster_v4(dst + (((c4 + g) ^ ((uint32_t)e_halo_slot & 7u)) << 4),
-                                          make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]));
+                        for (int i = 0; i < 8; ++i) {
+                            if (col0 + i * 8 >= L.n_pad) break;
+                            if (e_valid[h])
+                                *reinterpret_cast<uint32_t*>(smem + CH_OFF_ACT + boff + w_slot * 128 + (((uint32_t)i ^ ((uint32_t)w_slot & 7u)) << 4) + cp * 2) =
+                                    pk[ps][8 * h + i];
+                            if (e_halo[h] && !last)
+                                st_cluster_u32(peer_act + boff + (uint32_t)e_halo_slot[h] * 128u + (((uint32_t)i ^ ((uint32_t)e_halo_slot[h] & 7u)) << 4) + cp * 2,
+                                               pk[ps][8 * h + i]);
+                        }
                     }
                 }
                 if (tr0) CH_TRACE(4, l);
-                tc_fence_before();
                 if (!last) {
                     // padding slots the in-place operand tiles have overwritten: zero again for the next layer's depthwise
                     if ((int)threadIdx.x < nzc) {
@@ -445,7 +387,7 @@ chain_tc_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ 
                 fence_proxy_async();        // these generic-proxy writes precede async-proxy accesses (MMA reads, the next image's TMA)
                 __syncwarp();
                 if (lane == 0) mbar_arrive(smem_u32(&bars->aff_empty[as]));
-                // every local worker has left the epilogue (TMEM drained, activations written, halo row stored into the peer) ...
+                // every local worker has left the epilogue (activations written, halo row stored into the peer) ...
                 asm volatile("bar.sync %0, %1;" ::"r"(3), "r"(CH_WORKERS * 32) : "memory");
                 // ... so ONE cluster-scope release (MEMBAR.GPU class, ~500 cycles) publishes all sixteen warps' halo stores: the
                 // barrier orders them before this thread, and a release is cumulative
@@ -468,12 +410,7 @@ chain_tc_kernel(const __grid_constant__ ChainMaps maps, const __grid_constant__ 
     }
 
     __syncwarp();
-    tc_fence_before();
-    cluster_sync_all();                            // nobody exits (or frees TMEM) while the peer may still touch this CTA
-    if (warp == CH_WARP_MMA) {
-        tc_fence_after();
-        tmem_dealloc_2cta(tmem_base, 512u);
-    }
+    cluster_sync_all();                            // nobody exits while the peer may still touch this CTA
 }
 
 // ----------------------------------------------------------------------------------------------------------
@@ -573,7 +510,7 @@ int chain_tc_prepare(int dtype, const BlockArgs* layers, int n_layers, const TcL
         L.c_in = g.c_in; L.c_out = g.c_out;
         L.kblocks = (g.c_in + 63) / 64;
         L.n_pad = (g.c_out + 31) / 32 * 32;
-        L.nh = (L.n_pad + 255) / 256;
+        L.np = (L.n_pad + 127) / 128;
         L.aff_bytes = L.n_pad * 8;
         void* dwp = nullptr; float2* aff = nullptr;
         if (cudaMalloc(&dwp, (size_t)L.kblocks * CH_DWP) != cudaSuccess || cudaMalloc(&aff, (size_t)L.n_pad * sizeof(float2)) != cudaSuccess) {

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the fastdepth_b200 kernels (sm_100a only).
+// Shared device/host helpers for the fastdepth_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -8,8 +8,8 @@
 
 #include "../../include/fastdepth_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "fastdepth_b200 targets sm_100a only (-gencode arch=compute_100a,code=sm_100a)"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "fastdepth_b200 targets sm_90a only (-gencode arch=compute_90a,code=sm_90a)"
 #endif
 
 namespace fd {
@@ -124,7 +124,7 @@ struct StageGeom {
 struct TcLaunchOpts {
     int pdl = 1;             // programmatic dependent launch attribute on every launch
     int sleep_ns = 0;        // > 0: latency-tolerant mbarrier waits back off with nanosleep instead of spinning
-    int n_sms = 148;         // SMs of the plan's device (grid size and the planner's wave model)
+    int n_sms = 132;         // SMs of the plan's device (grid size and the planner's wave model)
     int cluster = 1;         // 1: the block planner may run small-map blocks on thread-block clusters that share the depthwise half
 };
 

@@ -8,7 +8,7 @@
 //                                                                      (reference models.py:698,731)
 //
 // dw_kernel + pw_kernel are "path 0": the unfused, reference-quality implementation every
-// dtype can run (it is the fp32 path and the on-device cross-check for the fused tcgen05
+// dtype can run (it is the fp32 path and the on-device cross-check for the fused wgmma
 // block kernel in fd_block_tc.cu).  All accumulate in fp32 and apply BN as a folded fp32
 // per-channel affine, then round once to the storage dtype.
 #include "fd_common.cuh"

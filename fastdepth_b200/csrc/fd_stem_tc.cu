@@ -1,14 +1,14 @@
-// Stem (conv_bn(3, C0, stride 2) + BN + ReLU6, reference imagenet/mobilenet.py:22-27, 41) on tcgen05.
+// Stem (conv_bn(3, C0, stride 2) + BN + ReLU6, reference imagenet/mobilenet.py:22-27, 41) on wgmma.
 //
 // A dense 3x3x3 convolution is a K = 27 contraction per output pixel: on SIMT that is 27*C0 FMAs per pixel
-// (694 MMAC per batch of 64, more than twice the HBM time of the stage), on the tensor core it is one
-// M=128 x N=C0 x K=32 UMMA per 128-pixel tile once the im2col rows sit in shared memory.  So:
+// (694 MMAC per batch of 64, more than twice the HBM time of the stage), on the tensor core it is a
+// M=128 x N=C0 x K=32 product per 128-pixel tile once the im2col rows sit in shared memory.  So:
 //   warp 8     TMA producer : 4-D box [1 img][3 planes][17 rows][40 cols] of the NCHW input per 8x16 output tile
 //                             (OOB zero fill == the conv's zero padding); stem weights [C0pad x 64] loaded once
 //   warps 0-3  im2col       : thread = output pixel; gathers its 27 taps from the staged planes and writes the
 //                             128B-swizzled K-major A row (K padded to 32 with zeros)
-//   warp 9     MMA issuer   : two K=16 tcgen05.mma per tile into a double-buffered TMEM accumulator
-//   warps 4-7  epilogue     : tcgen05.ld -> BN affine + ReLU6 -> 16-bit NHWC store
+//   warps 4-7  consumer     : one warpgroup: wgmma m64n32k16 (two row halves x C0 / 32 column blocks x two K steps) into
+//                             register accumulators -> BN affine + ReLU6 -> 16-bit NHWC store
 // Persistent: one CTA per SM walks tiles blockIdx.x, +gridDim.x, ...
 #include <cstdio>
 #include <cstring>
@@ -19,7 +19,8 @@
 
 namespace fd {
 
-constexpr int ST_WARP_EPI0 = 4, ST_WARP_TMA = 8, ST_WARP_MMA = 9, ST_THREADS = 320;
+constexpr int ST_WARP_EPI0 = 4, ST_WARP_TMA = 8, ST_THREADS = 288;
+constexpr int ST_MAX_N = 64;                          // output channels the register accumulators hold
 constexpr int ST_TH = 8, ST_TW = 16;
 constexpr int ST_IH = 17, ST_IW = 40;                 // rows 2*7+3 = 17; cols: the 33 needed ones sit at box columns 7..39 because
                                                       // the box starts 8 elements (16 bytes) left of column 2*ox0 (aligned start)
@@ -30,10 +31,9 @@ constexpr int ST_A_BYTES = 128 * 128;
 constexpr int ST_S_IN = 8, ST_S_A = 3;
 
 struct StemParams {
-    int n, h_in, w_in, h_out, w_out, c_out, n_pad;   // n_pad: c_out rounded up to 16
+    int n, h_in, w_in, h_out, w_out, c_out, n_pad;   // n_pad: c_out rounded up to 32 (one wgmma column block)
     int out_pitch;                                   // elements between output pixels (>= c_out)
     int tiles_x, tiles_y, items;
-    int tmem_cols;
     unsigned long long mg_tx, mg_ty;
     void* out;
     const float2* affine;    // [n_pad / 2] x (scale, scale, bias, bias) of a channel pair
@@ -42,9 +42,7 @@ struct StemParams {
 struct StemBarriers {
     uint64_t in_full[ST_S_IN], in_empty[ST_S_IN];
     uint64_t a_full[ST_S_A], a_empty[ST_S_A];
-    uint64_t acc_full[2], acc_empty[2];
     uint64_t b_full;
-    uint32_t tmem_base, pad;
 };
 
 template <typename T>
@@ -66,20 +64,15 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
     if (threadIdx.x == 0) {
         for (int i = 0; i < ST_S_IN; ++i) { mbar_init(smem_u32(&bars->in_full[i]), 1); mbar_init(smem_u32(&bars->in_empty[i]), 4); }
         for (int i = 0; i < ST_S_A; ++i) { mbar_init(smem_u32(&bars->a_full[i]), 4); mbar_init(smem_u32(&bars->a_empty[i]), 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(smem_u32(&bars->acc_full[i]), 1); mbar_init(smem_u32(&bars->acc_empty[i]), 4); }
         mbar_init(smem_u32(&bars->b_full), 1);
         fence_barrier_init();
     }
-    if (warp == ST_WARP_MMA) tmem_alloc(smem_u32(&bars->tmem_base), (uint32_t)p.tmem_cols);
     if (warp == ST_WARP_TMA && lane == 0) { tma_prefetch_desc(&tm_in); tma_prefetch_desc(&tm_w); }
     for (int i = threadIdx.x; i < p.n_pad; i += ST_THREADS) s_affine[i] = p.affine[i];
     // the K = 32..63 half of every A row is never read (only two K=16 steps are issued), no need to clear it
     pdl_launch_dependents();                       // the next kernel may begin its own prologue
     pdl_wait_prior_grid();                         // everything below reads what the previous kernel wrote
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = bars->tmem_base;
 
     auto decode = [&](int w, int& img, int& oy0, int& ox0) {
         const uint32_t t2 = fdiv40((uint32_t)w, p.mg_tx);
@@ -100,26 +93,6 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
                 mbar_wait(smem_u32(&bars->in_empty[rin.s]), rin.ph ^ 1u);
                 mbar_expect_tx(smem_u32(&bars->in_full[rin.s]), ST_IN_BYTES);
                 tma_load_4d(smem_base + in_off + rin.s * ST_IN_STRIDE, &tm_in, smem_u32(&bars->in_full[rin.s]), 2 * ox0 - ST_XSHIFT, 2 * oy0 - 1, 0, img);
-            }
-        }
-    } else if (warp == ST_WARP_MMA) {
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | (MF::kUmmaFormat << 7) | (MF::kUmmaFormat << 10) | ((128u >> 4) << 24) |
-                                   ((uint32_t)(p.n_pad >> 3) << 17);
-            mbar_wait(smem_u32(&bars->b_full), 0);
-            tc_fence_after();
-            const uint64_t b_desc = make_kmajor_sw128_desc(smem_base + b_off);
-            Ring ra, racc;
-            for (int w = blockIdx.x; w < p.items; w += gridDim.x, ra.next(ST_S_A), racc.next(2)) {
-                mbar_wait(smem_u32(&bars->acc_empty[racc.s]), racc.ph ^ 1u);
-                mbar_wait(smem_u32(&bars->a_full[ra.s]), ra.ph);
-                tc_fence_after();
-                const uint64_t a_desc = make_kmajor_sw128_desc(smem_base + a_off + ra.s * ST_A_BYTES);
-                const uint32_t d_tmem = tmem_base + racc.s * (uint32_t)p.n_pad;
-                umma_f16(d_tmem, a_desc, b_desc, idesc, 0u);
-                umma_f16(d_tmem, a_desc + 2, b_desc + 2, idesc, 1u);
-                umma_commit(smem_u32(&bars->a_empty[ra.s]));
-                umma_commit(smem_u32(&bars->acc_full[racc.s]));
             }
         }
     } else if (warp < ST_WARP_EPI0) {
@@ -159,53 +132,53 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
             if (lane == 0) mbar_arrive(smem_u32(&bars->a_full[ra.s]));
         }
     } else {
-        // =========================== epilogue ===========================
-        const int q = warp - ST_WARP_EPI0;
-        const int m = q * 32 + lane;
-        const int ty = m / ST_TW, tx = m % ST_TW;
+        // =========================== consumer warpgroup: wgmma + epilogue ===========================
+        const int wq = warp - ST_WARP_EPI0, cq = (lane & 3) * 2;
         T* __restrict__ outp = reinterpret_cast<T*>(p.out);
-        const int batches = (p.n_pad + 31) >> 5;
-        Ring racc;
-        for (int w = blockIdx.x; w < p.items; w += gridDim.x, racc.next(2)) {
+        const int nch = p.n_pad >> 5;                    // 32-column blocks
+        mbar_wait(smem_u32(&bars->b_full), 0);
+        const uint32_t b_lo = sw128_desc_lo(smem_base + b_off);
+        Ring ra;
+        for (int w = blockIdx.x; w < p.items; w += gridDim.x, ra.next(ST_S_A)) {
             int img, oy0, ox0;
             decode(w, img, oy0, ox0);
-            const int oy = oy0 + ty, ox = ox0 + tx;
-            const bool valid = oy < p.h_out && ox < p.w_out;
-            mbar_wait(smem_u32(&bars->acc_full[racc.s]), racc.ph);
-            tc_fence_after();
-            const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16) + racc.s * (uint32_t)p.n_pad;
-            T* o = outp + (((size_t)img * p.h_out + oy) * p.w_out + ox) * p.out_pitch;
-            for (int b = 0; b < batches; ++b) {
-                uint32_t r[32];
-                const bool full = b * 32 + 32 <= p.n_pad;
-                if (full) tmem_ld32_sync(t_lane + b * 32, r);
-                else tmem_ld16_sync(t_lane + b * 32, r);
+            float acc[2][ST_MAX_N / 32][16];              // [row half][column block]
+            mbar_wait(smem_u32(&bars->a_full[ra.s]), ra.ph);
+            const uint32_t a_lo = sw128_desc_lo(smem_base + a_off + ra.s * ST_A_BYTES);
+            wgmma_fence();
 #pragma unroll
-                for (int g = 0; g < 4; ++g) {                  // 8 channels = one 16-byte store
-                    if (g >= 2 && !full) break;
-                    const int c0 = b * 32 + g * 8;
-                    uint32_t pk[4];
+            for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float4 af = *reinterpret_cast<const float4*>(s_affine + c0 + 2 * j);     // (s0, s1, b0, b1)
-                        pk[j] = MF::template pack_act<true>(ffma2_abc(
-                            f32x2_make(__uint_as_float(r[g * 8 + 2 * j]), __uint_as_float(r[g * 8 + 2 * j + 1])),
-                            f32x2_make(af.x, af.y), f32x2_make(af.z, af.w)));
+                for (int j = 0; j < ST_MAX_N / 32; ++j) {
+                    if (j < nch) {                        // K = 32: two steps of 16 (+32 B each); B rows of block j at +j * 4 KB
+                        wgmma_n32<T>(acc[mh][j], sw128_desc(a_lo + (uint32_t)mh * 512u), sw128_desc(b_lo + (uint32_t)j * 256u), 0u);
+                        wgmma_n32<T>(acc[mh][j], sw128_desc(a_lo + (uint32_t)mh * 512u + 2u), sw128_desc(b_lo + (uint32_t)j * 256u + 2u), 1u);
                     }
-                    if (valid && c0 + 8 <= p.c_out) *reinterpret_cast<uint4*>(o + c0) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
                 }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&bars->acc_empty[racc.s]));
+            wgmma_commit();
+            wgmma_wait0();
+            if (wq == 0 && lane == 0) mbar_arrive(smem_u32(&bars->a_empty[ra.s]));
+#pragma unroll
+            for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = mh * 64 + wq * 16 + (lane >> 2) + 8 * h;     // pixel of the tile
+                    const int oy = oy0 + m / ST_TW, ox = ox0 + m % ST_TW;
+                    if (oy >= p.h_out || ox >= p.w_out) continue;
+                    T* o = outp + (((size_t)img * p.h_out + oy) * p.w_out + ox) * p.out_pitch;
+#pragma unroll
+                    for (int j = 0; j < ST_MAX_N / 32; ++j)
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const int c0 = j * 32 + i * 8;            // 8-channel group; this thread's pair is c0 + cq
+                            if (j < nch && c0 < p.c_out) {
+                                const float4 af = *reinterpret_cast<const float4*>(s_affine + c0 + cq);     // (s0, s1, b0, b1)
+                                *reinterpret_cast<uint32_t*>(o + c0 + cq) = MF::template pack_act<true>(ffma2_abc(
+                                    f32x2_make(acc[mh][j][4 * i + 2 * h], acc[mh][j][4 * i + 2 * h + 1]), f32x2_make(af.x, af.y), f32x2_make(af.z, af.w)));
+                            }
+                        }
+                }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == ST_WARP_MMA) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
     }
 }
 
@@ -236,7 +209,7 @@ __global__ void pack_stem_w_kernel(const float* __restrict__ w27, T* __restrict_
 __global__ void pack_stem_affine_kernel(const float* __restrict__ scale, const float* __restrict__ bias, float2* __restrict__ dst,
                                         int c_out, int n_pad) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    // per channel PAIR (2j, 2j+1): (scale, scale, bias, bias), one 16-byte load feeds an FFMA2 (same layout as the block kernel)
+    // per channel PAIR (2j, 2j+1): (scale, scale, bias, bias), one 16-byte load feeds the pair (same layout as the block kernel)
     if (i < n_pad) {
         float* d = reinterpret_cast<float*>(dst) + (i >> 1) * 4;
         d[i & 1] = i < c_out ? scale[i] : 0.f;
@@ -247,7 +220,7 @@ __global__ void pack_stem_affine_kernel(const float* __restrict__ scale, const f
 bool stem_tc_supported(int dtype, const StageGeom& g) {
     if (dtype != FD_F16 && dtype != FD_BF16) return false;
     if (g.ksize != 3 || g.stride != 2 || g.c_in != 3 || g.act != FD_ACT_RELU6) return false;
-    if (g.c_out % 8 || g.c_out > 256 || (g.w_in % 8)) return false;       // W*2 bytes must be a 16-byte multiple for TMA
+    if (g.c_out % 8 || g.c_out > ST_MAX_N || (g.w_in % 8)) return false;       // W*2 bytes must be a 16-byte multiple for TMA
     return get_tensor_map_encoder() != nullptr;
 }
 
@@ -281,12 +254,10 @@ int stem_tc_prepare(int dtype, const StageGeom& g, const float* w27_dev, const f
     StemParams& p = sp->p;
     memset(&p, 0, sizeof(p));
     p.n = g.n; p.h_in = g.h_in; p.w_in = g.w_in; p.h_out = g.h_out; p.w_out = g.w_out; p.c_out = g.c_out;
-    p.n_pad = (g.c_out + 15) / 16 * 16;
+    p.n_pad = (g.c_out + 31) / 32 * 32;
     p.out_pitch = g.out_pitch > 0 ? g.out_pitch : g.c_out;
     p.tiles_x = (g.w_out + ST_TW - 1) / ST_TW; p.tiles_y = (g.h_out + ST_TH - 1) / ST_TH;
     p.items = p.tiles_x * p.tiles_y * g.n;
-    p.tmem_cols = 32;
-    while (p.tmem_cols < 2 * p.n_pad) p.tmem_cols *= 2;
     auto magic = [](int d) { return (unsigned long long)((1ULL << 40) / (unsigned long long)d) + 1ULL; };
     p.mg_tx = magic(p.tiles_x); p.mg_ty = magic(p.tiles_y);
     p.out = out;

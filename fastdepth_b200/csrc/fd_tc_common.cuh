@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA / mbarrier PTX wrappers shared by the sm_100a tensor-core kernels
+// wgmma / TMA / mbarrier / cluster PTX wrappers shared by the sm_90a tensor-core kernels
 // (fd_block_tc.cu: fused depthwise->pointwise blocks; fd_stem_tc.cu: im2col stem).
 #pragma once
 #include <cuda.h>
@@ -23,8 +23,8 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
 // Blocking wait with a suspend-time hint: the thread is parked by the hardware (no issue slots burnt) until the phase
-// completes or the hint (ns) expires, instead of spinning on short default time-outs -- in the ncu instruction mix of the
-// hint-less version 40 % of all issued warp-instructions of decode_conv5 were TRYWAIT/BRA/YIELD of waiting warps.
+// completes or the hint (ns) expires, instead of spinning on short default time-outs, so that waiting warps take few issue slots
+// from the warps that compute.
 #ifdef FD_TC_WATCHDOG
 // Debug build (-DFD_TC_WATCHDOG): every blocking barrier wait gives up after ~50 ms, reports who waited for what and traps, so a
 // protocol dead-lock shows up as a launch failure with a message instead of a hung GPU.
@@ -52,10 +52,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "WAIT_DONE:\n\t}" ::"r"(bar), "r"(parity), "r"(1000000u) : "memory");
 }
 #endif
-// Wait for roles that can afford wake-up latency (epilogue warps waiting for an accumulator, the TMA producer waiting for
-// a free stage).  ncu's source view of conv7 showed mbar_wait's try_wait/NANOSLEEP.SYNCS pair re-issuing every ~27 cycles
-// per waiting warp whatever the suspend hint says -- a quarter of all warp instructions of the kernel, taken from the
-// schedulers the depthwise warps issue on.  A plain timed sleep between probes really parks the warp.
+// Wait for roles that can afford wake-up latency (the TMA producer waiting for a free stage): a plain timed sleep between
+// probes parks the warp whatever the hardware does with the suspend-time hint.
 __device__ __forceinline__ void mbar_wait_sleep(uint32_t bar, uint32_t parity, uint32_t ns) {
     if (ns == 0u) { mbar_wait(bar, parity); return; }
     for (;;) {
@@ -69,11 +67,8 @@ __device__ __forceinline__ void mbar_wait_sleep(uint32_t bar, uint32_t parity, u
     }
 }
 // A plain probe loop with a pause between probes, used by the tile-sharing cluster instance of the block kernel (its waiters
-// sit on barriers that are completed from OTHER SMs: bulk-copy bytes, multicast commits).  Bring-up record: forced onto multi-wave
-// launches that instance stalls with the hinted wait, with this loop and with back-to-back probes alike (8 of 8 runs), while the
-// library built with -DFD_TC_WATCHDOG (same loop plus a clock read per probe) ran through 4 of 4 times with correct results --
-// a timing-dependent interaction that is NOT root-caused; the planner therefore admits that mode on one-wave launches only
-// (FD_TC_CLUSTER_MULTIWAVE=1 lifts the limit for further bring-up).
+// sit on barriers that are completed from OTHER SMs: bulk-copy bytes, remote arrivals).  The planner admits that mode on
+// one-wave launches only (FD_TC_CLUSTER_MULTIWAVE=1 lifts the limit for experiments).
 __device__ __forceinline__ void mbar_wait_nohint(uint32_t bar, uint32_t parity) {
 #ifdef FD_TC_WATCHDOG
     mbar_wait(bar, parity);          // the watchdog form is a plain probe loop already
@@ -97,8 +92,6 @@ __device__ __forceinline__ void mbar_wait_sleep_sel(uint32_t bar, uint32_t parit
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
     asm volatile(
@@ -139,78 +132,45 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, both operands K-major, 16-bit inputs, fp32 accumulate
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc),
-        "r"(accumulate) : "memory");
-}
-// same, descriptors given as 32-bit halves (the high word of a K-major SW128 descriptor is a constant)
-__device__ __forceinline__ void umma_f16_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi, uint32_t idesc,
-                                              uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tmov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\tsetp.ne.b32 p, %5, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t}" ::"r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc),
-        "r"(accumulate) : "memory");
-}
-constexpr uint32_t kSw128DescHi = (1024u >> 4) | (1u << 14) | (2u << 29);      // SBO = 1024 B, version 1, SWIZZLE_128B
+// ---- Hopper warpgroup MMA (wgmma): D[regs] (+)= A[smem] * B[smem]^T, both operands K-major 128B-swizzled, fp32 accumulate.
+// A warpgroup (four consecutive warps, the first one's id a multiple of four) computes a 64-row slice; thread t of it holds rows
+// 16 * (t / 32) + (t % 32) / 4 (+ 8) and, per 8-column group j, the columns 8 j + 2 (t % 4) (+ 1):
+//   d[4 j + 0], d[4 j + 1] = row r, columns c, c + 1;   d[4 j + 2], d[4 j + 3] = row r + 8, same columns.
+// K-major, SWIZZLE_128B shared-memory matrix descriptor: start address >> 4, LBO (unused for swizzled K-major) = 1, SBO = 1024 B
+// between 8-row groups, layout type 1 (128B swizzle) in bits 62-63.  The start address advances by 32 B (2 in the low word) per
+// K step of 16 elements inside the 128-byte swizzle row.
+constexpr uint32_t kSw128DescHi = (1024u >> 4) | (1u << 30);
 __device__ __forceinline__ uint32_t sw128_desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3FFFu) | (1u << 16); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-}
-// 32 consecutive columns of this thread's TMEM lane, load + wait in ONE asm statement so that no use of the
-// destination registers can be scheduled before tcgen05.wait::ld
-__device__ __forceinline__ void tmem_ld32_sync(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16_sync(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-}
-// split issue / wait so that the next TMEM load can be in flight while the previous batch is being processed.  The wait
-// lists the destination registers as read-write operands: no use of them can be scheduled above it.
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait_regs(uint32_t (&r)[32]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31]) :: "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait_regs16(uint32_t (&r)[32]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]) :: "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ uint64_t sw128_desc(uint32_t lo) { return ((uint64_t)kSw128DescHi << 32) | lo; }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+#define FD_WGMMA_N64(TY)                                                                                                        \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                                          \
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " "                                                   \
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,"  \
+                 "%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"                                                                  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),    \
+                   "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),         \
+                   "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),        \
+                   "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])                      \
+                 : "l"(a), "l"(b), "r"(acc))
+#define FD_WGMMA_N32(TY)                                                                                                        \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"                                                          \
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " "                                                   \
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"                      \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),    \
+                   "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])                       \
+                 : "l"(a), "l"(b), "r"(acc))
+// m64 x n64 x k16 (or n32), accumulate when acc != 0, else overwrite
+template <typename T> __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc);
+template <> __device__ __forceinline__ void wgmma_n64<__half>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) { FD_WGMMA_N64("f16"); }
+template <> __device__ __forceinline__ void wgmma_n64<__nv_bfloat16>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) { FD_WGMMA_N64("bf16"); }
+template <typename T> __device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc);
+template <> __device__ __forceinline__ void wgmma_n32<__half>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) { FD_WGMMA_N32("f16"); }
+template <> __device__ __forceinline__ void wgmma_n32<__nv_bfloat16>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) { FD_WGMMA_N32("bf16"); }
+#undef FD_WGMMA_N64
+#undef FD_WGMMA_N32
 
 // ---- thread-block clusters: rank, cluster barrier, DSMEM addresses, remote mbarrier arrives ---------------
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
@@ -222,14 +182,6 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
 }
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
     asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// Remote arrive WITHOUT a cluster-scope release: `mbarrier.arrive.release.cluster` compiles to MEMBAR.ALL.GPU + ERRBAR (a
-// quarter of the worker warps' time in the first version of this kernel, ncu source page of profiles/r02_v1_*).  It is used
-// where the data the arrival publishes lives in the ARRIVING CTA's own shared memory and is read there by that CTA's half of
-// the tensor-core pair: the writes were already made visible to the async proxy by fence.proxy.async (which completes them),
-// only the signal crosses to the leader.
-__device__ __forceinline__ void mbar_arrive_remote_cta_scope(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cta.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 // wait on a LOCAL barrier whose arrivals come (also) from the peer CTA: acquire at cluster scope
 __device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity, uint32_t ns) {
@@ -250,39 +202,18 @@ __device__ __forceinline__ void bulk_copy_to_peer(uint32_t dst_cluster, uint32_t
     asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst_cluster), "r"(src_cta), "r"(bytes), "r"(bar_cluster) : "memory");
 }
-// tcgen05.commit of a one-CTA MMA stream arriving on the barrier at the same shared-memory offset in EVERY CTA of `mask`
-__device__ __forceinline__ void umma_commit_multicast(uint32_t bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_100 UMMA): start address >> 4, LBO (unused for
-// swizzled K-major) = 1, SBO = 1024 B between 8-row groups, descriptor version 1, layout type 2 (128B swizzle).
-__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-// Packed fp32 pair (channel pair of one lane) and the Blackwell two-wide FMA, SASS FFMA2: one instruction, two FMAs.  It
-// does not raise FMA throughput (32 lanes x 2 takes the pipe two cycles) but halves the instructions issued; used for the
-// BN affine of channel pairs everywhere and for the 3x3 depthwise inner product (tools/fma2_tput*.cu, DESIGN.md section 7).
-// Results are bit-identical to FHFMA: a 16-bit x 16-bit product is exact in the fp32 FMA either way.
+// Packed fp32 pair (channel pair of one lane).  The pair travels as one 64-bit value and is computed as two FMAs; a 16-bit x
+// 16-bit product is exact in fp32, so widening first and using the fp32 FMA gives the mixed-precision result bit for bit.
 typedef unsigned long long f32x2;
-__device__ __forceinline__ void ffma2(f32x2& acc, f32x2 a, f32x2 b) { asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b)); }
-__device__ __forceinline__ f32x2 ffma2_abc(f32x2 a, f32x2 b, f32x2 c) {
-    f32x2 d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
-}
 __device__ __forceinline__ f32x2 f32x2_make(float lo, float hi) { return ((f32x2)__float_as_uint(hi) << 32) | (f32x2)__float_as_uint(lo); }
 __device__ __forceinline__ float f32x2_lo(f32x2 v) { return __uint_as_float((uint32_t)v); }
 __device__ __forceinline__ float f32x2_hi(f32x2 v) { return __uint_as_float((uint32_t)(v >> 32)); }
+__device__ __forceinline__ f32x2 ffma2_abc(f32x2 a, f32x2 b, f32x2 c) {
+    return f32x2_make(fmaf(f32x2_lo(a), f32x2_lo(b), f32x2_lo(c)), fmaf(f32x2_hi(a), f32x2_hi(b), f32x2_hi(c)));
+}
+__device__ __forceinline__ void ffma2(f32x2& acc, f32x2 a, f32x2 b) { acc = ffma2_abc(a, b, acc); }
 
-// mixed-precision FMA: exact 16-bit x 16-bit product added into fp32 (SASS FHFMA / FHFMA.BF16)
+// mixed-precision FMA: exact 16-bit x 16-bit product added into fp32
 template <typename T> struct MixFma;
 template <> struct MixFma<__half> {
     __device__ __forceinline__ static f32x2 widen(uint32_t v) {           // two HADD2.F32
@@ -290,8 +221,9 @@ template <> struct MixFma<__half> {
         return f32x2_make(f.x, f.y);
     }
     __device__ __forceinline__ static void fma2(float& lo, float& hi, uint32_t a, uint32_t b) {
-        asm("{\n\t.reg .f16 al, ah, bl, bh;\n\tmov.b32 {al, ah}, %2;\n\tmov.b32 {bl, bh}, %3;\n\t"
-            "fma.rn.f32.f16 %0, al, bl, %0;\n\tfma.rn.f32.f16 %1, ah, bh, %1;\n\t}" : "+f"(lo), "+f"(hi) : "r"(a), "r"(b));
+        const f32x2 x = widen(a), y = widen(b);
+        lo = fmaf(f32x2_lo(x), f32x2_lo(y), lo);
+        hi = fmaf(f32x2_hi(x), f32x2_hi(y), hi);
     }
     __device__ __forceinline__ static uint32_t pack(float lo, float hi) {
         __half2 h = __floats2half2_rn(lo, hi);
@@ -307,15 +239,15 @@ template <> struct MixFma<__half> {
         if (RELU6) asm("min.f16x2 %0, %0, %1;" : "+r"(h) : "r"(0x46004600u));
         return h;
     }
-    static constexpr uint32_t kUmmaFormat = 0;   // F16
 };
 template <> struct MixFma<__nv_bfloat16> {
     __device__ __forceinline__ static f32x2 widen(uint32_t v) {           // bf16 -> fp32 is a 16-bit shift
         return f32x2_make(__uint_as_float(v << 16), __uint_as_float(v & 0xffff0000u));
     }
     __device__ __forceinline__ static void fma2(float& lo, float& hi, uint32_t a, uint32_t b) {
-        asm("{\n\t.reg .b16 al, ah, bl, bh;\n\tmov.b32 {al, ah}, %2;\n\tmov.b32 {bl, bh}, %3;\n\t"
-            "fma.rn.f32.bf16 %0, al, bl, %0;\n\tfma.rn.f32.bf16 %1, ah, bh, %1;\n\t}" : "+f"(lo), "+f"(hi) : "r"(a), "r"(b));
+        const f32x2 x = widen(a), y = widen(b);
+        lo = fmaf(f32x2_lo(x), f32x2_lo(y), lo);
+        hi = fmaf(f32x2_hi(x), f32x2_hi(y), hi);
     }
     __device__ __forceinline__ static uint32_t pack(float lo, float hi) {
         __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
@@ -329,7 +261,6 @@ template <> struct MixFma<__nv_bfloat16> {
         if (RELU6) asm("min.bf16x2 %0, %0, %1;" : "+r"(h) : "r"(0x40C040C0u));
         return h;
     }
-    static constexpr uint32_t kUmmaFormat = 1;   // BF16
 };
 
 // programmatic dependent launch: let the next kernel of the stream start its prologue on SMs this grid has already left,
@@ -345,7 +276,7 @@ struct Ring {
 // exact w / d for w, d < 2^20 with mg = floor(2^40 / d) + 1
 __device__ __forceinline__ uint32_t fdiv40(uint32_t w, unsigned long long mg) { return (uint32_t)(((unsigned long long)w * mg) >> 40); }
 
-// scalar BN affine + activation (head path only; the block paths do channel PAIRS: FFMA2 + MixFma::pack_act)
+// scalar BN affine + activation (head path only; the block paths do channel PAIRS: ffma2_abc + MixFma::pack_act)
 template <bool RELU6>
 __device__ __forceinline__ float affine_act(float acc, float s, float b) {
     const float v = fmaxf(fmaf(acc, s, b), 0.0f);

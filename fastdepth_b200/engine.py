@@ -103,11 +103,11 @@ class ForwardLanes:
     CUDA stream and its own C-ABI host pipeline (``fd_pipeline_submit`` / ``fd_pipeline_wait``) -- that take batches round-robin.
 
     One forward is a chain of 15 persistent kernels with one 227 KB CTA per SM, so at every kernel boundary the SMs that finish early
-    idle until the next kernel has filled its pipeline (about 6 us per boundary, 15 % of the step).  A second and third batch in flight
-    on other streams fill those gaps with their own kernels: 594 -> 537 (two lanes) -> 520 us per batch of 64 (three lanes) on one B200.
+    idle until the next kernel has filled its pipeline.  A second and third batch in flight
+    on other streams fill those gaps with their own kernels.
     The module's own ``forward`` keeps strict single-stream semantics (and the lowest latency); this class is for serving loops that
     have several batches to run and only care when each one is done.  (Programmatic dependent launch stays off on the lanes: its
-    early-launched dependents hold SMs that another lane's kernel could use -- 531 vs 520 us with three lanes.)
+    early-launched dependents hold SMs that another lane's kernel could use.)
     """
 
     def __init__(self, module, lanes=3, options=None):

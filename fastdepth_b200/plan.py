@@ -240,12 +240,11 @@ class Plan:
                 lo, hi = st['kernel'].split('{stages ')[1].rstrip('}').split('-')
                 in_chain = in_chain or int(lo) <= stage <= int(hi)
         if in_chain:
-            cnames = ('layer_start', 'dw_first_kb_computed', 'dw_done_grp0', 'acc_full_seen', 'epilogue_done', 'local_barrier',
-                      'halo_received', 'mma_first_a_full', 'mma_last_commit', 'dw_done_grp1', 'tma_first_b_issue',
-                      'mma_first_b_full')
+            cnames = ('layer_start', 'dw_first_kb_computed', 'dw_done_grp0', 'pointwise_done', 'epilogue_done', 'local_barrier',
+                      'halo_received', 'mma_first_a_full', 'mma_last_pass_done', 'dw_done_grp1', 'tma_first_b_issue', 'unused11')
             return {n: a[i][a[i] > 0] for i, n in enumerate(cnames)}
-        names = ('tma_issue', 'dw_start', 'dw_math_done', 'a_published', 'mma_ready', 'mma_issued', 'epi_start', 'epi_done',
-                 'epi_tmem_loaded', 'epi_staged', 'epi_barrier', 'epi_store_issued')
+        names = ('tma_issue', 'dw_start', 'dw_math_done', 'a_published', 'mma_ready', 'mma_issued', 'unused6', 'epi_done',
+                 'unused8', 'epi_staged', 'epi_barrier', 'epi_store_issued')
         return {n: a[i][a[i] > 0] for i, n in enumerate(names)}
 
     def stage_tensor(self, stage, which=0):  # noqa: C901

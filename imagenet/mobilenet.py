@@ -11,7 +11,7 @@ State-dict keys are identical to the reference (``model.<i>.<0|1|3|4>.*``,
 ``fc.*``) so ImageNet checkpoints written by the reference load unchanged.
 Nothing here runs on the hot path: on CUDA the blocks are *read* by
 ``fastdepth_b200.plan`` (conv weight + BN statistics) and executed by the
-sm_100a kernels.
+sm_90a kernels.
 
 Extension over the reference: ``widths`` lets callers build NetAdapt-pruned
 encoders (SURVEY.md section 8a-a10); the default reproduces the stock widths.

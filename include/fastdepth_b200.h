@@ -1,5 +1,5 @@
 /*
- * fastdepth_b200 -- C-ABI of the B200-native FastDepth forward path.
+ * fastdepth_b200 -- C-ABI of the H100-native FastDepth forward path.
  *
  * This is the drop-in boundary for ONE hot path of dwofk/fast-depth:
  *     MobileNetSkipAdd.forward            (reference models.py:706-732)
@@ -95,7 +95,7 @@ int fd_plan_set_stage_weights(fd_plan* plan, int stage,
                               const float* pw_w, const float* pw_scale, const float* pw_bias);
 
 /* Tunables, by name.  Unknown names fail with FD_ERR_INVALID.
- *   "path"       0 = SIMT reference-quality kernels (all dtypes), 1 = fused tcgen05 block
+ *   "path"       0 = SIMT reference-quality kernels (all dtypes), 1 = fused wgmma block
  *                kernels where available (16-bit dtypes)            [default 1]
  *   "fold_head"  1 = apply decode_conv6 below the last upsample (exact: 1x1 conv/BN/ReLU
  *                commute with nearest upsampling, SURVEY.md section 2b row 8) [default 1]
@@ -106,9 +106,7 @@ int fd_plan_set_stage_weights(fd_plan* plan, int stage,
  *                after fd_forward (set 0 for stage-by-stage inspection)  [default 1]
  *   "pdl"        1 = tensor-core kernels are launched with programmatic dependent launch so that each
  *                kernel's prologue overlaps the previous kernel's tail.  With one 227 KB CTA per SM the early-launched
- *                dependents mostly hold SMs idle while they wait for the previous grid: measured 596.8 us per forward
- *                with it, 589.4 us without (round 2), and it costs more when several plans run concurrently
- *                [default 0]
+ *                dependents mostly hold SMs idle while they wait for the previous grid  [default 0]
  *   "chain"      1 = a run of consecutive 3x3 stride-1 blocks on a small feature map (conv7..conv11 at 14x14) executes as ONE
  *                kernel on 2-CTA clusters with every intermediate activation resident in shared memory; the intermediate
  *                stages' buffers are then not written (set 0 for stage-by-stage inspection)  [default 1]
@@ -116,9 +114,9 @@ int fd_plan_set_stage_weights(fd_plan* plan, int stage,
  *                each CTA computes the depthwise half of a quarter (half) of the K-blocks, broadcasts its operand tiles to
  *                the others through distributed shared memory and runs the MMAs of one output-channel split (chosen by
  *                the planner's cost model for the small-map, many-channel blocks)  [default 1]
- *   "wait_sleep_ns" > 0: latency-tolerant roles of the fused block kernel (epilogue warps waiting for an
- *                accumulator, TMA producer waiting for a free stage) sleep this many ns between barrier
- *                probes instead of spinning (measured: no effect on B200, the spinning waiters do not
+ *   "wait_sleep_ns" > 0: latency-tolerant roles of the fused block kernel (the TMA producer waiting for a
+ *                free stage) sleep this many ns between barrier
+ *                probes instead of spinning (the spinning waiters do not
  *                take issue slots the depthwise warps could use)  [default 0]   */
 int fd_plan_set_option(fd_plan* plan, const char* name, int value);
 int fd_plan_get_option(fd_plan* plan, const char* name, int* value);
@@ -176,10 +174,8 @@ int fd_plan_trace_stage(fd_plan* plan, int stage, void* y_dev, void* stream,
                         unsigned long long* out_host, int cap, int* rows, int* cols);
 
 /* Debug (host only, needs no GPU): the shared-memory / pipeline plan the fused block kernel would use for one
- * block.  out[0..15] = {ok, splits, n_cta, items, kblocks, s_in, s_a, s_b, bn, nb, b_resident, epi_groups, n_stg,
- * smem_bytes, tmem_cols, in_stage_stride}; with cap >= 18 also out[16..17] = {nacc (TMEM accumulators), epi_colsplit},
- * with cap >= 19 out[18] = epi_wide, with cap >= 20 out[19] = cs (cluster size: CTAs sharing one tile's depthwise half), with cap >= 21 out[20] = dw_teams.
- * cap must be at least 16. */
+ * block.  out[0..15] = {ok, splits, n_cta, items, kblocks, s_in, s_a, s_b, bn, nb, b_resident, n_stg, smem_bytes,
+ * in_stage_stride, cs (cluster size: CTAs sharing one tile's depthwise half), dw_teams}.  cap must be at least 16. */
 int fd_debug_block_plan(int ksize, int stride, int h_out, int w_out, int n, int c_in, int c_out, int head,
                         int* out, int cap);
 

@@ -1,11 +1,11 @@
-"""FastDepth model surface, B200-native.
+"""FastDepth model surface, H100-native.
 
 This module keeps the *names* the reference harness and its pickled
 checkpoints resolve (``models.MobileNetSkipAdd``, ``models.MobileNet``,
 ``models.choose_decoder``, ``models.weights_init`` ... -- reference
 models.py:36-75, 224-270, 335-360, 420-460, 654-732) while the forward of the
 hot path, ``MobileNetSkipAdd.forward`` (reference models.py:706-732), is
-executed by hand-written sm_100a kernels behind the C-ABI in
+executed by hand-written sm_90a kernels behind the C-ABI in
 ``include/fastdepth_b200.h``.
 
 What is here and what is not (SURVEY.md section 2 / section 8):
@@ -133,7 +133,7 @@ def choose_decoder(decoder):
         model = NNConv(int(decoder[6]), use_dw)
     elif any(decoder.startswith(p) for p in _OUT_OF_SCOPE_DECODERS):
         raise NotImplementedError(
-            "decoder '%s' is out of scope of the B200 hot-path build (only nnconv*); see DESIGN.md" % decoder)
+            "decoder '%s' is out of scope of the H100 hot-path build (only nnconv*); see DESIGN.md" % decoder)
     else:
         assert False, "invalid option for decoder: {}".format(decoder)
     model.apply(weights_init)
@@ -172,7 +172,7 @@ class MobileNet(nn.Module):
     def forward(self, x):
         """CPU tensors (BASELINE config 1 plumbing) and the dense 5x5 decoder run on stock PyTorch, exactly like the
         reference (models.py:457-460).  A CUDA tensor through the depthwise NNConv decoder ("MobileNet-NNConv5(dw)",
-        reference README.md:37) takes the same fused sm_100a path as MobileNetSkipAdd, just without skips."""
+        reference README.md:37) takes the same fused sm_90a path as MobileNetSkipAdd, just without skips."""
         fused_ok = (x.is_cuda and not self.training and x.dim() == 4 and x.shape[1] == 3 and
                     x.shape[2] % 32 == 0 and x.shape[3] % 32 == 0)     # what the fused plan covers; anything else: stock PyTorch
         if fused_ok:

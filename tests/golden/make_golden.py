@@ -1,15 +1,15 @@
 """Generate the golden fixtures in this directory FROM THE LIVE REFERENCE.
 
-Run in the build container (the only place /root/reference exists):
+Run with a checkout of the reference (dwofk/fast-depth) at hand:
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py /path/to/fast-depth
 
 It imports the reference's own ``models.py`` / ``metrics.py`` read-only under alias module
 names (the repo has same-named top-level modules), instantiates the reference's
 ``MobileNetSkipAdd`` (models.py:654-732), loads the seeded synthetic state_dict from
 ``fastdepth_b200.synthetic`` and records the reference forward's outputs.  Nothing from the
-reference is copied: only numbers it computed.  The GPU box has no /root/reference; the
-tests there read the committed .npz files.
+reference is copied: only numbers it computed.  The tests read the committed .npz files and
+never need the reference itself.
 """
 import importlib.util
 import os
@@ -21,7 +21,7 @@ import torch.nn as nn
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = '/root/reference'
+REF = os.path.abspath(sys.argv[1]) if len(sys.argv) > 1 else None
 sys.path.insert(0, ROOT)
 
 from fastdepth_b200 import synthetic  # noqa: E402
@@ -31,7 +31,7 @@ N_SAMPLE = 96
 
 
 def load_reference():
-    """Load /root/reference/{models,metrics}.py as ref_models / ref_metrics.  The reference does
+    """Load the reference's {models,metrics}.py as ref_models / ref_metrics.  The reference does
     ``import imagenet.mobilenet`` (models.py:8), so point those names at ITS copies meanwhile."""
     saved = {k: sys.modules.get(k) for k in ('imagenet', 'imagenet.mobilenet', 'models', 'metrics')}
     for k in saved:
@@ -189,6 +189,8 @@ def make_metrics_fixture(ref_metrics):
 
 
 if __name__ == '__main__':
+    if REF is None:
+        raise SystemExit('usage: make_golden.py <path of a dwofk/fast-depth checkout>')
     torch.manual_seed(0)
     torch.set_num_threads(8)
     ref_models, ref_metrics = load_reference()

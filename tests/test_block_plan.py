@@ -1,21 +1,22 @@
 """Host-only check of the fused block kernel's shared-memory / pipeline planner (no GPU needed): every block of
 the stock and the NetAdapt-pruned network, at 224x224 b64, 480x640 b16 and tiny shapes, must get a plan that fits
-the 227 KB of a B200 SM, keeps the TMEM accumulator pair within 512 columns and never falls back to narrow MMAs."""
+the 227 KB of an H100 SM, keeps an item's register accumulator within 128 columns, uses whole 64- or 128-row weight stages and
+at most the two staging tiles the kernel alternates between."""
 import ctypes
 
 import pytest
 
 from fastdepth_b200 import _lib, synthetic
 
-KEYS = ('ok', 'splits', 'n_cta', 'items', 'kblocks', 's_in', 's_a', 's_b', 'bn', 'nb', 'b_resident', 'epi_groups',
-        'n_stg', 'smem_bytes', 'tmem_cols', 'in_stage_stride', 'nacc', 'epi_colsplit', 'epi_wide', 'cs', 'dw_teams')
+KEYS = ('ok', 'splits', 'n_cta', 'items', 'kblocks', 's_in', 's_a', 's_b', 'bn', 'nb', 'b_resident', 'n_stg',
+        'smem_bytes', 'in_stage_stride', 'cs', 'dw_teams')
 STRIDES = (2, 1, 2, 1, 2, 1, 2, 1, 1, 1, 1, 1, 2, 1)
 
 
 def plan(ks, stride, h, w, n, cin, cout, head=0):
     lib = _lib.load()
-    out = (ctypes.c_int * 21)()
-    _lib.check(lib.fd_debug_block_plan(ks, stride, h, w, n, cin, cout, head, out, 21))
+    out = (ctypes.c_int * 16)()
+    _lib.check(lib.fd_debug_block_plan(ks, stride, h, w, n, cin, cout, head, out, 16))
     return dict(zip(KEYS, out))
 
 
@@ -39,14 +40,11 @@ def test_every_block_gets_a_valid_plan(built_lib, widths, shape):
         p = plan(ks, stride, hh, ww, n, cin, cout, head)
         assert p['ok'] == 1, (name, p)
         assert p['smem_bytes'] <= 227 * 1024, (name, p)
-        assert p['nacc'] in (1, 2) and p['nacc'] * p['n_cta'] <= p['tmem_cols'] <= 512 and p['n_cta'] % 16 == 0, (name, p)
-        assert p['nacc'] == 2 or (p['epi_colsplit'] == 1 and p['epi_groups'] == 2), (name, p)   # one accumulator: both groups drain it
-        assert not p['epi_colsplit'] or (p['epi_groups'] == 2 and p['n_cta'] > 64 and not head), (name, p)
+        assert p['n_cta'] % 16 == 0 and p['n_cta'] <= 128 and p['bn'] in (64, 128), (name, p)   # register accumulators, wgmma blocks
         assert p['n_cta'] * p['splits'] >= cout and (p['splits'] == 1 or p['n_cta'] % 64 == 0), (name, p)
         assert p['s_in'] >= 1 and 2 <= p['s_a'] <= (6 if p['cs'] > 1 else 4) and p['bn'] * p['nb'] >= p['n_cta'], (name, p)
-        assert p['cs'] == 1 or (p['cs'] in (2, 4) and p['splits'] == p['cs'] and p['kblocks'] >= p['cs'] and p['nacc'] == 2 and not head), (name, p)
-        assert p['bn'] >= min(64, p['n_cta']), (name, p)            # no narrow MMAs
-        assert p['epi_groups'] in (1, 2) and (head or p['n_stg'] in (p['epi_groups'], 2 * p['epi_groups'])), (name, p)
+        assert p['cs'] == 1 or (p['cs'] in (2, 4) and p['splits'] == p['cs'] and p['kblocks'] >= p['cs'] and not head), (name, p)
+        assert p['n_stg'] == 0 if head else p['n_stg'] in (1, 2), (name, p)
         if p['b_resident']:
             assert p['splits'] == 1 and p['s_b'] == p['kblocks'] * p['nb'] <= 16
 
@@ -54,10 +52,10 @@ def test_every_block_gets_a_valid_plan(built_lib, widths, shape):
 def test_stock_b64_plans_snapshot(built_lib):
     """The metric configuration: high-res blocks keep their weights resident and a deep A ring."""
     p = plan(3, 1, 112, 112, 64, 32, 64)          # conv1
-    assert p['b_resident'] == 1 and p['s_a'] == 4 and p['epi_groups'] == 2 and p['items'] == 6272
+    assert p['b_resident'] == 1 and p['s_a'] == 4 and p['n_stg'] == 2 and p['items'] == 6272
     p = plan(3, 1, 14, 14, 64, 512, 512)          # conv7..11
-    # one 512-column accumulator per tile: the depthwise half and the input tile are not repeated per split
-    assert p['splits'] == 1 and p['n_cta'] == 512 and p['nacc'] == 1 and p['bn'] == 256 and p['epi_colsplit'] == 1
+    # an item's accumulator lives in registers: at most 128 channels, so four splits of one full-width weight stage each
+    assert p['splits'] == 4 and p['n_cta'] == 128 and p['bn'] == 128 and p['nb'] == 1
     p = plan(5, 1, 112, 112, 64, 64, 32, head=1)  # decode_conv5 + folded head
     assert p['n_stg'] == 0 and p['splits'] == 1 and p['dw_teams'] == 2       # one K-block, even rings: two depthwise teams
     p = plan(5, 1, 7, 7, 64, 1024, 512)           # decode_conv1: 32 tiles x 4 CTAs in one wave share the 5x5 depthwise half
@@ -87,25 +85,18 @@ def test_planner_invariants_on_random_blocks(built_lib):
         assert p['smem_bytes'] <= 227 * 1024, ctx
         assert p['n_cta'] % 16 == 0 and p['n_cta'] * p['splits'] >= cout, ctx
         assert p['splits'] == 1 or p['n_cta'] % 64 == 0, ctx                       # a TMA store box must not reach into the next split
-        assert p['nacc'] in (1, 2) and p['nacc'] * p['n_cta'] <= p['tmem_cols'] <= 512, ctx
-        assert p['tmem_cols'] >= 32 and p['tmem_cols'] & (p['tmem_cols'] - 1) == 0, ctx
-        assert p['bn'] % 16 == 0 and p['bn'] <= 256 and p['bn'] * p['nb'] >= p['n_cta'] > p['bn'] * (p['nb'] - 1), ctx
+        assert p['n_cta'] <= 128 and p['bn'] in (64, 128) and p['bn'] * p['nb'] >= p['n_cta'] > p['bn'] * (p['nb'] - 1), ctx
         assert p['kblocks'] == (cin + 63) // 64 and 2 <= p['s_a'] <= (6 if p['cs'] > 1 else 4) and 1 <= p['s_in'] <= 6, ctx
         # cluster mode: one split per CTA of the cluster, every CTA owns a K-block and a non-empty split, two accumulators
-        assert p['cs'] == 1 or (p['cs'] in (2, 4) and p['splits'] == p['cs'] and p['kblocks'] >= p['cs'] and p['nacc'] == 2 and
+        assert p['cs'] == 1 or (p['cs'] in (2, 4) and p['splits'] == p['cs'] and p['kblocks'] >= p['cs'] and
                                 p['n_cta'] * (p['cs'] - 1) < cout and not head), ctx
-        assert p['s_in'] >= 2 or (p['kblocks'] == 1 and p['items'] <= 148), ctx
+        assert p['s_in'] >= 2 or (p['kblocks'] == 1 and p['items'] <= 132), ctx
         assert 1 <= p['s_b'] <= 16 and (not p['b_resident'] or p['s_b'] == p['kblocks'] * p['nb']), ctx
-        assert p['epi_groups'] in (1, 2), ctx
         if head:
-            assert p['n_stg'] == 0 and p['splits'] == 1 and not p['epi_colsplit'] and not p['epi_wide'], ctx
+            assert p['n_stg'] == 0 and p['splits'] == 1, ctx
         else:
-            assert p['n_stg'] in (p['epi_groups'], 2 * p['epi_groups']), ctx
-            assert not p['epi_colsplit'] or (p['epi_groups'] == 2 and p['n_cta'] > 64), ctx
-            assert not p['epi_wide'] or p['epi_groups'] == 1, ctx
-            assert p['nacc'] == 2 or p['epi_colsplit'], ctx                        # one accumulator: both groups must drain it
-        assert p['nacc'] == 2 or p['items'] <= 148, ctx                            # ... and no CTA runs two items on it
-        assert p['cs'] == 1 or p['items'] <= 148, ctx                              # tile-sharing clusters: one wave only
+            assert p['n_stg'] in (1, 2), ctx                                       # the kernel alternates between at most two tiles
+        assert p['cs'] == 1 or p['items'] <= 132, ctx                              # tile-sharing clusters: one wave only
         assert p['dw_teams'] in (1, 2) and (p['dw_teams'] == 1 or (p['cs'] == 1 and p['s_in'] % 2 == 0 and p['s_a'] % 2 == 0)), ctx
 
     check()

@@ -1,5 +1,5 @@
 """A/B planner experiment knobs (environment variables read when a plan is built) on the bench workload.
-usage: python tools/ab_env.py "FD_TC_MAX_NCTA=256,FD_TC_NO_COLSPLIT=1" "FD_TC_MAX_NCTA=256" "" """
+usage: python tools/ab_env.py "FD_TC_MAX_NCTA=64,FD_TC_CLUSTER=1" "FD_TC_MAX_NCTA=64" "" """
 import sys, os
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -14,7 +14,7 @@ y = torch.empty((64, 1, 224, 224), dtype=torch.half, device='cuda')
 sp = torch.cuda.current_stream().cuda_stream
 ref = None
 for cfg in sys.argv[1:]:
-    for k in ('FD_TC_MAX_NCTA', 'FD_TC_NO_COLSPLIT', 'FD_TC_NO_WIDE'):
+    for k in ('FD_TC_MAX_NCTA', 'FD_TC_CLUSTER'):
         os.environ.pop(k, None)
     for kv in filter(None, cfg.split(',')):
         k, v = kv.split('='); os.environ[k] = v

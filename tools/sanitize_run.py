@@ -1,7 +1,7 @@
 """Small-shape workload for compute-sanitizer (memcheck / racecheck / synccheck / initcheck) over every kernel organisation
 of the fused path: stock and pruned widths, fp16 and bf16, TMA and LSU epilogues, in-place skip accumulation on and off, head
-folded and not, the planner's epilogue organisations (environment knobs), graph replay and direct launches.
-usage (on the GPU box): compute-sanitizer --tool memcheck python tools/sanitize_run.py [quick]"""
+folded and not, the planner's output-channel splits (environment knobs), graph replay and direct launches.
+usage (on a machine with an H100 and compute-sanitizer): compute-sanitizer --tool memcheck python tools/sanitize_run.py [quick]"""
 import itertools
 import os
 import sys
@@ -24,10 +24,10 @@ for widths, wname in ((synthetic.STOCK_WIDTHS, 'stock'), (synthetic.PRUNED_WIDTH
             m = m.eval().cuda().to(dtype)
             x = synthetic.synthetic_input(n, h, w, seed=3).cuda().to(dtype)
             ref = {}
-            envs = ({}, {'FD_TC_MAX_NCTA': '128', 'FD_TC_NO_COLSPLIT': '1', 'FD_TC_NO_WIDE': '1'})
+            envs = ({}, {'FD_TC_MAX_NCTA': '64', 'FD_TC_CLUSTER': '1'})
             for env, (tma, inpl, fold, graph) in itertools.product(envs if not quick else envs[:1],
                                                                    ((1, 1, 1, 0), (1, 0, 0, 0), (0, 0, 1, 0), (1, 1, 1, 1))):
-                for k in ('FD_TC_MAX_NCTA', 'FD_TC_NO_COLSPLIT', 'FD_TC_NO_WIDE'):
+                for k in ('FD_TC_MAX_NCTA', 'FD_TC_CLUSTER'):
                     os.environ.pop(k, None)
                 os.environ.update(env)
                 eng = SkipAddEngine(m)

@@ -1,4 +1,4 @@
-"""Timeline of the chain kernel (leader CTA of cluster 0, first image): per-layer SM-clock stamps of the roles."""
+"""Timeline of the chain kernel (CTA 0 of cluster 0, first image): per-layer SM-clock stamps of the roles."""
 import os, sys
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -24,8 +24,8 @@ for k, v in tr.items():
     print('%-22s %s' % (k, ' '.join('%7d' % (a - t0) for a in v)))
 ls, le = tr['layer_start'] - t0, tr['halo_received'] - t0
 print('per layer (cycles):', ' '.join('%d' % (b - a) for a, b in zip(ls, le)))
-for a, b, n in (('layer_start', 'dw_done_grp0', 'dw phase grp0'), ('dw_done_grp0', 'acc_full_seen', 'wait for MMAs'),
-                ('acc_full_seen', 'epilogue_done', 'epilogue'), ('epilogue_done', 'local_barrier', 'zero list + local barrier'),
+for a, b, n in (('layer_start', 'dw_done_grp0', 'dw phase grp0'), ('dw_done_grp0', 'pointwise_done', 'pointwise passes'),
+                ('pointwise_done', 'epilogue_done', 'epilogue'), ('epilogue_done', 'local_barrier', 'zero list + local barrier'),
                 ('local_barrier', 'halo_received', 'halo wait')):
     n_ = min(len(tr[a]), len(tr[b]))
     print('%-28s %s' % (n, ' '.join('%6d' % d for d in (tr[b][:n_] - tr[a][:n_]))))
