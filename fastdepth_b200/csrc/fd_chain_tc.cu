@@ -69,7 +69,7 @@ struct ChainLayer {
     int c_in, c_out;
     int kblocks;           // ceil(c_in / 64)
     int np;                // passes of 128 output channels: ceil(n_pad / 128)
-    int n_pad;             // c_out rounded up to 32 (accumulator columns in use)
+    int n_pad;             // c_out rounded up to 64 (accumulator columns in use; every written K-block is whole)
     int aff_bytes;         // n_pad * 8
     const void* dwp;       // [kblocks] x CH_DWP bytes
     const float2* affine;  // [n_pad]: (scale, scale, bias, bias) per channel PAIR (see pack_affine_kernel)
@@ -509,7 +509,10 @@ int chain_tc_prepare(int dtype, const BlockArgs* layers, int n_layers, const TcL
         ChainLayer& L = p.L[l];
         L.c_in = g.c_in; L.c_out = g.c_out;
         L.kblocks = (g.c_in + 63) / 64;
-        L.n_pad = (g.c_out + 31) / 32 * 32;
+        // whole 64-channel blocks: the epilogue then writes every channel of the next layer's last K-block (zeros past c_out), so
+        // its depthwise never reads shared memory this launch did not write (0 x a leftover Inf would be NaN).  The wgmma is n64
+        // either way, so the padding costs no MMA work.
+        L.n_pad = (g.c_out + 63) / 64 * 64;
         L.np = (L.n_pad + 127) / 128;
         L.aff_bytes = L.n_pad * 8;
         void* dwp = nullptr; float2* aff = nullptr;
