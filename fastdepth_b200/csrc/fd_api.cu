@@ -7,11 +7,13 @@
 #include <vector>
 
 #include "fd_block_plan.h"
+#include "fd_conv_plan.h"
 #include "fd_common.cuh"
 
 namespace fd {
 
 BlockPlanOut block_tc_debug_plan(int ksize, int stride, int h_out, int w_out, int n, int c_in, int c_out, int head);
+ConvPlanOut conv_tc_debug_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms);
 
 // ---- error state -----------------------------------------------------------------------
 static thread_local std::string g_last_error;
@@ -26,6 +28,8 @@ int launch_stem(int dtype, const void* x, void* out, const float* w, const float
                 const StageGeom& g, cudaStream_t st);
 int launch_dw(int dtype, const BlockArgs& a, cudaStream_t st);
 int launch_pw(int dtype, const BlockArgs& a, cudaStream_t st);
+int launch_conv(int dtype, const void* in, const void* w, void* out, const float* scale, const float* bias, const StageGeom& g,
+                cudaStream_t st);
 int launch_head(int dtype, const void* in, void* out, const float* w, float scale, float bias, long long m_total, int c,
                 int in_pitch, int h, int wd, int up, int act, cudaStream_t st);
 int launch_metrics(int dtype, const void* pred, const float* target, int n, int hw, double* sums, cudaStream_t st);
@@ -56,6 +60,14 @@ int stem_tc_prepare(int dtype, const StageGeom& g, const float* w27_dev, const f
 int stem_tc_launch(StemTcPlan* sp, const void* x, cudaStream_t st);
 void stem_tc_destroy(StemTcPlan* sp);
 const char* stem_tc_name(StemTcPlan* sp);
+// dense kxk conv on wgmma (fd_conv_tc.cu)
+struct ConvTcPlan;
+bool conv_tc_supported(int dtype, const StageGeom& g);
+int conv_tc_prepare(int dtype, const StageGeom& g, const void* in, const void* w, const float* scale_dev, const float* bias_dev,
+                    void* out, const TcLaunchOpts& opts, ConvTcPlan** res);
+int conv_tc_launch(ConvTcPlan* cp, cudaStream_t st);
+void conv_tc_destroy(ConvTcPlan* cp);
+const char* conv_tc_name(ConvTcPlan* cp);
 
 static size_t dtype_size(int dtype) { return dtype == FD_F32 ? 4 : 2; }
 
@@ -73,7 +85,7 @@ struct Stage {
     float* dw_w = nullptr;               // [k*k][c_in]
     float* dw_scale = nullptr;
     float* dw_bias = nullptr;
-    void* pw_w = nullptr;                // [c_out][c_in] plan dtype (DWPW)
+    void* pw_w = nullptr;                // [c_out][c_in] plan dtype (DWPW); [c_out][k*k][c_in] plan dtype (CONV)
     float* pw_w_f32 = nullptr;           // stem: [27][c_out] tap-major ; head: [c_in]
     float* pw_scale = nullptr;
     float* pw_bias = nullptr;
@@ -81,6 +93,7 @@ struct Stage {
     bool have_weights = false;
     BlockTcPlan* tc = nullptr;
     StemTcPlan* stc = nullptr;
+    ConvTcPlan* ctc = nullptr;
     ChainTcPlan* chain = nullptr;        // set on the FIRST stage of a run executed by the chain kernel
     int chained = 0;                     // 1: this stage runs inside a chain kernel (its own output buffer is only written if it is
                                          //    the run's last stage)
@@ -158,6 +171,7 @@ static void invalidate(fd_plan* p) {
     for (auto& s : p->stages) {
         if (s.tc) { block_tc_destroy(s.tc); s.tc = nullptr; }
         if (s.stc) { stem_tc_destroy(s.stc); s.stc = nullptr; }
+        if (s.ctc) { conv_tc_destroy(s.ctc); s.ctc = nullptr; }
         if (s.chain) { chain_tc_destroy(s.chain); s.chain = nullptr; }
         s.chained = 0;
     }
@@ -192,7 +206,8 @@ static int build_steps(fd_plan* p) {
     Stage& last = p->stages[ns - 2];
     // decode_conv6 below the last upsample: exact because a 1x1 conv, a per-channel affine and ReLU
     // act pixel-wise and nearest upsampling only replicates pixels (SURVEY.md section 2b row 8).
-    const bool fold = p->opt_fold_head && last.d.kind == FD_STAGE_DWPW && last.d.upsample && last.d.skip_src < 0;
+    const bool fold = p->opt_fold_head && (last.d.kind == FD_STAGE_DWPW || last.d.kind == FD_STAGE_CONV) && last.d.upsample &&
+                      last.d.skip_src < 0;
     bool head_fused = false;
 
     for (int i = 0; i < ns; ++i) {
@@ -220,6 +235,36 @@ static int build_steps(fd_plan* p) {
             } else {
                 st.run = [sp, dtype](cudaStream_t stream, const void* x, void*) {
                     return launch_stem(dtype, x, sp->out, sp->pw_w_f32, sp->pw_scale, sp->pw_bias, sp->g, stream);
+                };
+            }
+            p->steps.push_back(st);
+        } else if (s.d.kind == FD_STAGE_CONV) {
+            // dense kxk conv: one implicit-GEMM step (path 1: conv_tc_kernel, else the SIMT conv_kernel); with the head folded
+            // below the last upsample the stage stores at conv resolution and head_kernel<up2x> replicates
+            StageGeom g = s.g;
+            if (fold && &s == &last) g.upsample = 0;
+            const double px_in = (double)g.n * g.h_in * g.w_in, px_out = (double)g.n * g.h_out * g.w_out;
+            const double kk = (double)g.ksize * g.ksize;
+            Step st;
+            st.stage = i;
+            st.macs = px_out * g.c_in * g.c_out * kk;
+            st.dw_macs = 0.0;
+            st.alg_bytes = (px_in * g.c_in + px_out * (g.upsample ? 4.0 : 1.0) * g.c_out) * es + kk * g.c_in * g.c_out * es +
+                           2.0 * g.c_out * 4;
+            const int dtype = p->dtype;
+            if (p->opt_path == 1 && conv_tc_supported(dtype, g)) {
+                int rc = conv_tc_prepare(dtype, g, in, s.pw_w, s.pw_scale, s.pw_bias, s.out, lopts, &s.ctc);
+                if (rc != FD_OK) return rc;
+                st.name = conv_tc_name(s.ctc);
+                ConvTcPlan* ctc = s.ctc;
+                st.run = [ctc](cudaStream_t stream, const void*, void*) { return conv_tc_launch(ctc, stream); };
+            } else {
+                char nm[64];
+                snprintf(nm, sizeof(nm), "conv_kernel<k%d>", g.ksize);
+                st.name = nm;
+                Stage* sp = &s;
+                st.run = [sp, in, g, dtype](cudaStream_t stream, const void*, void*) {
+                    return launch_conv(dtype, in, sp->pw_w, sp->out, sp->pw_scale, sp->pw_bias, g, stream);
                 };
             }
             p->steps.push_back(st);
@@ -404,7 +449,8 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages, int n, int h, int 
         const fd_stage_desc& d = s.d;
         const bool first = i == 0, lastst = i == n_stages - 1;
         if ((d.kind == FD_STAGE_STEM) != first || (d.kind == FD_STAGE_HEAD) != lastst ||
-            (!first && !lastst && d.kind != FD_STAGE_DWPW)) { rc = fail(FD_ERR_INVALID, "stage list must be STEM, DWPW..., HEAD"); break; }
+            (!first && !lastst && d.kind != FD_STAGE_DWPW && d.kind != FD_STAGE_CONV)) {
+            rc = fail(FD_ERR_INVALID, "stage list must be STEM, (DWPW|CONV)..., HEAD"); break; }
         if (d.c_in != ch) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": c_in does not match producer"); break; }
         if (d.act != FD_ACT_RELU && d.act != FD_ACT_RELU6) { rc = fail(FD_ERR_INVALID, "bad act"); break; }
         s.g.n = n; s.g.h_in = hh; s.g.w_in = ww; s.g.c_in = d.c_in; s.g.c_out = d.c_out;
@@ -418,6 +464,12 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages, int n, int h, int 
                 rc = fail(FD_ERR_INVALID, "block stage needs k in {3,5}, stride 1|2, channels % 8 == 0"); break; }
             const int pad = (d.ksize - 1) / 2;
             s.g.h_out = (hh + 2 * pad - d.ksize) / d.stride + 1; s.g.w_out = (ww + 2 * pad - d.ksize) / d.stride + 1;
+        } else if (d.kind == FD_STAGE_CONV) {
+            if (d.skip_src >= 0) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": a CONV stage takes no skip"); break; }
+            if (d.stride != 1) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": a CONV stage has stride 1"); break; }
+            if ((d.ksize != 3 && d.ksize != 5) || d.c_in % 8 || d.c_out % 8 || d.c_out <= 0 || (d.upsample != 0 && d.upsample != 1)) {
+                rc = fail(FD_ERR_INVALID, "conv stage needs k in {3,5}, channels % 8 == 0, upsample 0|1"); break; }
+            s.g.h_out = hh; s.g.w_out = ww;
         } else {
             if (d.ksize != 1 || d.c_out != 1 || d.c_in % 8 || d.upsample || d.skip_src >= 0) {
                 rc = fail(FD_ERR_INVALID, "head must be 1x1, c_out 1, c_in % 8 == 0"); break; }
@@ -457,6 +509,8 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages, int n, int h, int 
             if ((rc = dev_alloc(p, (void**)&s.dw_scale, (size_t)d.c_in * 4))) break;
             if ((rc = dev_alloc(p, (void**)&s.dw_bias, (size_t)d.c_in * 4))) break;
             if ((rc = dev_alloc(p, &s.pw_w, (size_t)d.c_in * d.c_out * es))) break;
+        } else if (d.kind == FD_STAGE_CONV) {
+            if ((rc = dev_alloc(p, &s.pw_w, (size_t)d.ksize * d.ksize * d.c_in * d.c_out * es))) break;
         } else if (d.kind == FD_STAGE_STEM) {
             if ((rc = dev_alloc(p, (void**)&s.pw_w_f32, (size_t)27 * d.c_out * 4))) break;
         } else {
@@ -495,6 +549,14 @@ int fd_plan_set_stage_weights(fd_plan* p, int stage, const float* dw_w, const fl
         FD_CUDA_OK(cudaMemcpy(s.dw_scale, dw_scale, (size_t)d.c_in * 4, cudaMemcpyHostToDevice));
         FD_CUDA_OK(cudaMemcpy(s.dw_bias, dw_bias, (size_t)d.c_in * 4, cudaMemcpyHostToDevice));
         int rc = upload_as_dtype(p->dtype, pw_w, (size_t)d.c_in * d.c_out, s.pw_w);
+        if (rc) return rc;
+    } else if (d.kind == FD_STAGE_CONV) {
+        const int kk = d.ksize * d.ksize;
+        std::vector<float> t((size_t)d.c_out * kk * d.c_in);   // [co][ci][ky][kx] -> [co][(ky,kx)][ci]
+        for (int co = 0; co < d.c_out; ++co)
+            for (int ci = 0; ci < d.c_in; ++ci)
+                for (int j = 0; j < kk; ++j) t[((size_t)co * kk + j) * d.c_in + ci] = pw_w[((size_t)co * d.c_in + ci) * kk + j];
+        int rc = upload_as_dtype(p->dtype, t.data(), t.size(), s.pw_w);
         if (rc) return rc;
     } else if (d.kind == FD_STAGE_STEM) {
         std::vector<float> t((size_t)27 * d.c_out);            // [co][ci][ky][kx] -> [(ci,ky,kx)][co]
@@ -703,6 +765,7 @@ int fd_stage_buffer(fd_plan* p, int stage, int which, void** dev_ptr, int* n, in
         // with decode_conv6 folded below the last upsample the last block writes its low-res output
         if (p->opt_fold_head && stage == (int)p->stages.size() - 2 && s.d.upsample && s.d.skip_src < 0) { hh = s.g.h_out; ww = s.g.w_out; }
     } else if (which == 1) {
+        if (s.d.kind == FD_STAGE_CONV) return fail(FD_ERR_INVALID, "a CONV stage has no depthwise intermediate");
         ptr = s.mid; hh = s.g.h_out; ww = s.g.w_out; cc = s.g.c_in;
     } else {
         return fail(FD_ERR_INVALID, "which must be 0 or 1");
@@ -806,6 +869,7 @@ int fd_plan_trace_stage(fd_plan* p, int stage, void* y_dev, void* stream, unsign
     int rc = ensure_steps(p);
     if (rc) return rc;
     if (cap < 12 * 256) return fail(FD_ERR_INVALID, "trace buffer too small (need 3072 entries)");
+    if (p->stages[stage].d.kind == FD_STAGE_CONV) return fail(FD_ERR_INVALID, "the stage timeline exists for fused block kernels only");
     if (p->stages[stage].chain) return chain_tc_trace(p->stages[stage].chain, (cudaStream_t)stream, out_host, rows, cols);
     if (!p->stages[stage].tc) return fail(FD_ERR_STATE, "stage does not run the fused block kernel");
     return block_tc_trace(p->stages[stage].tc, (cudaStream_t)stream, y_dev, out_host, rows, cols);
@@ -816,6 +880,15 @@ int fd_debug_block_plan(int ksize, int stride, int h_out, int w_out, int n, int 
     const BlockPlanOut q = block_tc_debug_plan(ksize, stride, h_out, w_out, n, c_in, c_out, head);
     const int v[16] = {q.ok, q.splits, q.n_cta, q.items, q.kblocks, q.s_in, q.s_a, q.s_b, q.bn, q.nb, q.b_resident, q.n_stg,
                        q.smem_bytes, q.in_stage_stride, q.cs, q.dw_teams};
+    for (int i = 0; i < 16; ++i) out[i] = v[i];
+    return FD_OK;
+}
+
+int fd_debug_conv_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms, int* out, int cap) {
+    if (!out || cap < 16) return fail(FD_ERR_INVALID, "need an int[16] output");
+    const ConvPlanOut q = conv_tc_debug_plan(ksize, h_out, w_out, n, c_in, c_out, n_sms);
+    const int v[16] = {q.ok, q.ni, q.th, q.tw, q.bn, q.stages, q.m_tiles, q.n_splits, q.items, q.waves, q.kblocks, q.smem_bytes,
+                       q.useful_permille, (int)(q.cost > 2e9 ? 2e9 : q.cost), 0, 0};
     for (int i = 0; i < 16; ++i) out[i] = v[i];
     return FD_OK;
 }

@@ -1,0 +1,342 @@
+// Dense kxk stride-1 conv + folded BN + act (+ nearest x2 upsample) on wgmma: the conv() blocks of the dense NNConv decoder
+// (reference models.py:52-59, 245-270) as an implicit GEMM, M = output pixels, N = output channels, K = k*k*c_in.
+//
+// Work item = one tile of 128 output pixels (ni images x th rows x tw columns) times bn output channels (64, 128 or 256; see
+// fd_conv_plan.h for how the tile and bn are chosen).  The grid is one CTA per SM; every CTA walks items blockIdx.x,
+// +gridDim.x, ...  The K loop runs over (tap, 64-channel block):
+//   warp 8     TMA producer : per K step one 4-D box {64 ch, tw, th, ni} of the NHWC input, offset by (kx - p, ky - p), lands
+//                             128B-swizzled: every pixel's 64 channels are one 128-byte row, which IS the K-major SW128 A operand
+//                             (no im2col).  The OOB zero fill is the conv's zero padding and the channel tail.  Plus one box
+//                             {64 ch, 1 tap, bn rows} of the weights [c_out][k*k][c_in] (rows past c_out and channels past c_in
+//                             load as zeros)
+//   warps 0-7  consumers    : two warpgroups, each owning 64 of the 128 pixel rows: one wgmma m64 n(bn) k16 per 16 channels into
+//                             register accumulators, one commit group kept in flight; then BN affine + act -> 16-bit -> staging
+//                             tile -> TMA tensor stores (four strided views of the output for the nearest x2 upsample)
+// One mbarrier ring of operand stages (A + B) between the producer and the consumers.
+#include <cstdio>
+#include <cstring>
+#include <new>
+#include <string>
+
+#include "fd_conv_plan.h"
+#include "fd_tc_common.cuh"
+
+namespace fd {
+
+constexpr int CV_WARP_TMA = 8, CV_THREADS = 288;
+constexpr int CV_A_BYTES = 128 * 128;
+
+struct ConvParams {
+    int n, h, w, c_in, c_out;        // conv input == conv output size (stride 1, same padding)
+    int ni, th, tw;                  // tile: ni images x th rows x tw columns = 128 pixels
+    int tiles_x, tiles_y, splits, items;
+    int ks, pad, kblocks, ksteps;    // ksteps = ks * ks * kblocks
+    int stages, stage_bytes;
+    int upsample;
+    unsigned long long mg_splits, mg_tx, mg_ty;
+    const float2* affine;            // [splits * bn / 2] x (scale, scale, bias, bias) of a channel pair, zero padded
+};
+
+struct ConvBarriers {
+    uint64_t full[kConvMaxStages], empty[kConvMaxStages];
+};
+static_assert(sizeof(ConvBarriers) <= kConvBarrierBytes, "the planner budgets the barrier block");
+
+struct ConvCoord { int img0, oy0, ox0, n0; };
+__device__ __forceinline__ ConvCoord conv_decode(const ConvParams& p, int w, int bn) {
+    ConvCoord c;
+    const uint32_t t = fdiv40((uint32_t)w, p.mg_splits);
+    const int split = w - (int)t * p.splits;
+    const uint32_t t2 = fdiv40(t, p.mg_tx);
+    const int tx = (int)(t - t2 * (uint32_t)p.tiles_x);
+    const uint32_t t3 = fdiv40(t2, p.mg_ty);
+    const int ty = (int)(t2 - t3 * (uint32_t)p.tiles_y);
+    c.img0 = (int)t3 * p.ni; c.oy0 = ty * p.th; c.ox0 = tx * p.tw; c.n0 = split * bn;
+    return c;
+}
+
+template <typename T, int BN, bool RELU6>
+__global__ void __launch_bounds__(CV_THREADS, 1)
+conv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
+               const __grid_constant__ CUtensorMap tm_o0, const __grid_constant__ CUtensorMap tm_o1,
+               const __grid_constant__ CUtensorMap tm_o2, const __grid_constant__ CUtensorMap tm_o3, const ConvParams p) {
+    using MF = MixFma<T>;
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
+    // carve-up: [stages x (A 16 KB | B bn x 128 B)][2 staging tiles][barriers]; every piece a multiple of 1 KB
+    const uint32_t stg_off = (uint32_t)p.stages * (uint32_t)p.stage_bytes;
+    const uint32_t bar_off = stg_off + 2u * (uint32_t)kConvStg;
+    ConvBarriers* bars = reinterpret_cast<ConvBarriers*>(smem + bar_off);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < kConvMaxStages; ++i) { mbar_init(smem_u32(&bars->full[i]), 1); mbar_init(smem_u32(&bars->empty[i]), 2); }
+        fence_barrier_init();
+    }
+    if (warp == CV_WARP_TMA && lane == 0) {
+        tma_prefetch_desc(&tm_in); tma_prefetch_desc(&tm_w); tma_prefetch_desc(&tm_o0);
+        if (p.upsample) { tma_prefetch_desc(&tm_o1); tma_prefetch_desc(&tm_o2); tma_prefetch_desc(&tm_o3); }
+    }
+    pdl_launch_dependents();                       // the next kernel may begin its own prologue
+    pdl_wait_prior_grid();                         // everything below reads what the previous kernel wrote
+    __syncthreads();
+
+    if (warp == CV_WARP_TMA) {
+        // =========================== TMA producer ===========================
+        if (lane == 0) {
+            Ring r;
+            for (int w = blockIdx.x; w < p.items; w += gridDim.x) {
+                const ConvCoord c = conv_decode(p, w, BN);
+                for (int ky = 0; ky < p.ks; ++ky)
+                    for (int kx = 0; kx < p.ks; ++kx)
+                        for (int kb = 0; kb < p.kblocks; ++kb, r.next((uint32_t)p.stages)) {
+                            const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes, bar = smem_u32(&bars->full[r.s]);
+                            mbar_wait(smem_u32(&bars->empty[r.s]), r.ph ^ 1u);
+                            mbar_expect_tx(bar, (uint32_t)p.stage_bytes);
+                            tma_load_4d(st, &tm_in, bar, kb * 64, c.ox0 + kx - p.pad, c.oy0 + ky - p.pad, c.img0);
+                            tma_load_3d(st + CV_A_BYTES, &tm_w, bar, kb * 64, ky * p.ks + kx, c.n0);
+                        }
+            }
+        }
+    } else {
+        // =========================== consumer warpgroups: wgmma + epilogue ===========================
+        // warpgroup wg owns pixel rows [64 wg, 64 wg + 64) of every item; a thread holds rows r0 and r0 + 8 of every 8-column
+        // group j of the accumulator (fragment layout: see the wgmma wrappers)
+        const int wg = warp >> 2, wq = warp & 3;
+        const int r0 = wg * 64 + wq * 16 + (lane >> 2), cq = (lane & 3) * 2;
+        const bool leader = wq == 0 && lane == 0;          // releases this warpgroup's operand stages
+        const bool elected = warp == 0 && lane == 0;       // issues the tensor stores
+        constexpr uint32_t bar_id = 1u, bar_n = 256u;      // named barrier of the eight consumer warps
+        Ring r;
+        uint32_t stg_flip = 0;
+        for (int w = blockIdx.x; w < p.items; w += gridDim.x) {
+            const ConvCoord c = conv_decode(p, w, BN);
+            float acc[BN / 2];
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            uint32_t prev = 0;
+            for (int k = 0; k < p.ksteps; ++k) {
+                mbar_wait(smem_u32(&bars->full[r.s]), r.ph);
+                const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes;
+                const uint32_t a_lo = sw128_desc_lo(st + (uint32_t)wg * 8192u), b_lo = sw128_desc_lo(st + CV_A_BYTES);
+                wgmma_fence();
+#pragma unroll
+                for (int k4 = 0; k4 < 4; ++k4)             // +32 B (16 channels) per K step inside the 128-byte swizzle row
+                    wgmma_bn<T, BN>(acc, sw128_desc(a_lo + 2u * k4), sw128_desc(b_lo + 2u * k4), (k > 0 || k4 > 0) ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait1();                             // the previous step's MMAs are done: release its stage
+                if (k > 0 && leader) mbar_arrive(smem_u32(&bars->empty[prev]));
+                prev = r.s;
+                r.next((uint32_t)p.stages);
+            }
+            wgmma_wait0();
+            if (leader) mbar_arrive(smem_u32(&bars->empty[prev]));
+
+            // per block of 64 output channels: registers -> BN affine + act -> 16-bit -> shared staging tile [128 px][64 ch]
+            // (16-byte chunks XOR-swizzled like a SWIZZLE_128B box) -> TMA tensor stores; image borders and the channel tail
+            // are clipped by the hardware
+#pragma unroll
+            for (int cb = 0; cb < BN / 64; ++cb) {
+                if (c.n0 + cb * 64 >= p.c_out) break;
+                uint8_t* stg = smem + stg_off + (stg_flip & 1u) * (uint32_t)kConvStg;
+                ++stg_flip;
+                const float2* aff = p.affine + c.n0 + cb * 64;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {              // 8-column group i of this block: the thread's channel pair of rows r0, r0 + 8
+                    const float4 af = __ldg(reinterpret_cast<const float4*>(aff + i * 8 + cq));     // (s0, s1, b0, b1)
+                    const f32x2 sc = f32x2_make(af.x, af.y), bi = f32x2_make(af.z, af.w);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int rr = r0 + 8 * h;
+                        const int j = cb * 8 + i;
+                        *reinterpret_cast<uint32_t*>(stg + rr * 128 + ((i ^ (rr & 7)) << 4) + cq * 2) =
+                            MF::template pack_act<RELU6>(ffma2_abc(f32x2_make(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]), sc, bi));
+                    }
+                }
+                // before the OTHER staging buffer may be overwritten its previous store must have finished reading it
+                fence_proxy_async();
+                if (elected) bulk_wait_read0();
+                asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");
+                if (elected) {
+                    const uint32_t src = smem_u32(stg);
+                    const int cc = c.n0 + cb * 64;
+                    tma_store_4d(&tm_o0, src, cc, c.ox0, c.oy0, c.img0);
+                    if (p.upsample) {
+                        tma_store_4d(&tm_o1, src, cc, c.ox0, c.oy0, c.img0);
+                        tma_store_4d(&tm_o2, src, cc, c.ox0, c.oy0, c.img0);
+                        tma_store_4d(&tm_o3, src, cc, c.ox0, c.oy0, c.img0);
+                    }
+                    bulk_commit_group();
+                }
+            }
+        }
+        if (elected) bulk_wait_all();                      // all tensor stores have landed
+    }
+}
+
+// ----------------------------------------------------------------------------------------------
+// host side
+// ----------------------------------------------------------------------------------------------
+struct ConvTcPlan {
+    CUtensorMap tm_in, tm_w, tm_o[4];
+    ConvParams p;
+    ConvPlanOut po;
+    dim3 grid;
+    size_t smem_bytes;
+    int dtype, act;
+    TcLaunchOpts opts;
+    float2* affine = nullptr;
+    std::string name;
+};
+
+__global__ void pack_conv_affine_kernel(const float* __restrict__ scale, const float* __restrict__ bias, float2* __restrict__ dst,
+                                        int c_out, int n_pad) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    // per channel PAIR (2j, 2j+1): (scale, scale, bias, bias), one 16-byte load feeds the pair (same layout as the block kernel)
+    if (i < n_pad) {
+        float* d = reinterpret_cast<float*>(dst) + (i >> 1) * 4;
+        d[i & 1] = i < c_out ? scale[i] : 0.f;
+        d[2 + (i & 1)] = i < c_out ? bias[i] : 0.f;
+    }
+}
+
+bool conv_tc_supported(int dtype, const StageGeom& g) {
+    if (dtype != FD_F16 && dtype != FD_BF16) return false;
+    if ((g.ksize != 3 && g.ksize != 5) || g.stride != 1 || g.c_in % 8 || g.c_out % 8) return false;
+    return get_tensor_map_encoder() != nullptr;
+}
+
+void conv_tc_destroy(ConvTcPlan* cp) {
+    if (!cp) return;
+    cudaFree(cp->affine);
+    delete cp;
+}
+
+ConvPlanOut conv_tc_debug_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms) {
+    ConvPlanIn q{};
+    q.ksize = ksize; q.h_out = h_out; q.w_out = w_out; q.n = n; q.c_in = c_in; q.c_out = c_out; q.n_sms = n_sms;
+    q.force_tile = -1;
+    return plan_conv(q);
+}
+
+// FD_CONV_TILE=<index into kConvTiles> / FD_CONV_BN=64|128|256 pin the planner's choice (tests: the result must not depend on it)
+int conv_tc_prepare(int dtype, const StageGeom& g, const void* in, const void* w, const float* scale_dev, const float* bias_dev,
+                    void* out, const TcLaunchOpts& opts, ConvTcPlan** res) {
+    PFN_encodeTiled encode = get_tensor_map_encoder();
+    if (!encode) return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    ConvPlanIn q{};
+    q.ksize = g.ksize; q.h_out = g.h_out; q.w_out = g.w_out; q.n = g.n; q.c_in = g.c_in; q.c_out = g.c_out; q.upsample = g.upsample;
+    q.n_sms = opts.n_sms; q.force_tile = -1;
+    { const char* e = getenv("FD_CONV_TILE"); if (e && *e) q.force_tile = atoi(e); }
+    { const char* e = getenv("FD_CONV_BN"); if (e && *e) q.force_bn = atoi(e); }
+    const ConvPlanOut po = plan_conv(q);
+    if (!po.ok) return fail(FD_ERR_UNSUPPORTED, "dense conv stage: no tile plan fits shared memory");
+    ConvTcPlan* cp = new (std::nothrow) ConvTcPlan();
+    if (!cp) return fail(FD_ERR_CUDA, "out of host memory");
+    cp->dtype = dtype; cp->act = g.act; cp->opts = opts; cp->po = po;
+    ConvParams& p = cp->p;
+    memset(&p, 0, sizeof(p));
+    p.n = g.n; p.h = g.h_out; p.w = g.w_out; p.c_in = g.c_in; p.c_out = g.c_out;
+    p.ni = po.ni; p.th = po.th; p.tw = po.tw;
+    p.tiles_x = (g.w_out + po.tw - 1) / po.tw; p.tiles_y = (g.h_out + po.th - 1) / po.th;
+    p.splits = po.n_splits; p.items = po.items;
+    p.ks = g.ksize; p.pad = (g.ksize - 1) / 2; p.kblocks = po.kblocks; p.ksteps = g.ksize * g.ksize * po.kblocks;
+    p.stages = po.stages; p.stage_bytes = conv_stage_bytes(po.bn);
+    p.upsample = g.upsample;
+    auto magic = [](int d) { return (unsigned long long)((1ULL << 40) / (unsigned long long)d) + 1ULL; };
+    p.mg_splits = magic(p.splits); p.mg_tx = magic(p.tiles_x); p.mg_ty = magic(p.tiles_y);
+    const int n_pad = p.splits * po.bn;
+    if (cudaMalloc(&cp->affine, (size_t)n_pad * sizeof(float2)) != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cudaMalloc failed"); }
+    pack_conv_affine_kernel<<<(n_pad + 127) / 128, 128>>>(scale_dev, bias_dev, cp->affine, g.c_out, n_pad);
+    if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "conv affine packing failed"); }
+    p.affine = cp->affine;
+
+    const size_t es = 2;
+    const CUtensorMapDataType dt = dtype == FD_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    const int in_pitch = g.in_pitch > 0 ? g.in_pitch : g.c_in;
+    {   // input: NHWC viewed as (C, W, H, N); box (64, tw, th, ni); 128B swizzle == the wgmma A layout; OOB -> 0 (padding, channel tail)
+        cuuint64_t dims[4] = {(cuuint64_t)g.c_in, (cuuint64_t)g.w_in, (cuuint64_t)g.h_in, (cuuint64_t)g.n};
+        cuuint64_t strides[3] = {(cuuint64_t)in_pitch * es, (cuuint64_t)g.w_in * in_pitch * es, (cuuint64_t)g.h_in * g.w_in * in_pitch * es};
+        cuuint32_t box[4] = {64, (cuuint32_t)po.tw, (cuuint32_t)po.th, (cuuint32_t)po.ni};
+        cuuint32_t estr[4] = {1, 1, 1, 1};
+        CUresult r = encode(&cp->tm_in, dt, 4, const_cast<void*>(in), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(conv input) failed: " + std::to_string((int)r)); }
+    }
+    {   // weights [c_out][k*k][c_in] viewed as (C_in, taps, C_out); box (64, 1, bn) lands as bn K-major rows of 128 B
+        const int taps = g.ksize * g.ksize;
+        cuuint64_t dims[3] = {(cuuint64_t)g.c_in, (cuuint64_t)taps, (cuuint64_t)g.c_out};
+        cuuint64_t strides[2] = {(cuuint64_t)g.c_in * es, (cuuint64_t)taps * g.c_in * es};
+        cuuint32_t box[3] = {64, 1, (cuuint32_t)po.bn};
+        cuuint32_t estr[3] = {1, 1, 1};
+        CUresult r = encode(&cp->tm_w, dt, 3, const_cast<void*>(w), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(conv weights) failed: " + std::to_string((int)r)); }
+    }
+    // output views: plain NHWC, or the four (dy, dx) phases of the 2x nearest-upsampled tensor
+    memset(cp->tm_o, 0, sizeof(cp->tm_o));
+    {
+        const int up = g.upsample ? 2 : 1;
+        const cuuint64_t P = (cuuint64_t)(g.out_pitch > 0 ? g.out_pitch : g.c_out);
+        const cuuint64_t W2 = (cuuint64_t)g.w_out * up, H2 = (cuuint64_t)g.h_out * up;
+        for (int d = 0; d < (g.upsample ? 4 : 1); ++d) {
+            char* base = reinterpret_cast<char*>(out) + ((size_t)(d >> 1) * W2 + (d & 1)) * P * es;
+            cuuint64_t dims[4] = {(cuuint64_t)g.c_out, (cuuint64_t)g.w_out, (cuuint64_t)g.h_out, (cuuint64_t)g.n};
+            cuuint64_t strides[3] = {up * P * es, up * W2 * P * es, H2 * W2 * P * es};
+            cuuint32_t box[4] = {64, (cuuint32_t)po.tw, (cuuint32_t)po.th, (cuuint32_t)po.ni};
+            cuuint32_t estr[4] = {1, 1, 1, 1};
+            CUresult r = encode(&cp->tm_o[d], dt, 4, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(conv output) failed: " + std::to_string((int)r)); }
+        }
+    }
+    cp->smem_bytes = (size_t)po.smem_bytes;
+    cp->grid = dim3((unsigned)(p.items < opts.n_sms ? p.items : opts.n_sms), 1, 1);
+    char buf[160];
+    snprintf(buf, sizeof(buf), "conv_tc_kernel<k%d,bn%d,%s>[%dx%dx%d,n%d,st%d,%s]", g.ksize, po.bn, g.upsample ? "up" : "noup",
+             po.ni, po.th, po.tw, p.splits, p.stages, g.act == FD_ACT_RELU6 ? "relu6" : "relu");
+    cp->name = buf;
+    *res = cp;
+    return FD_OK;
+}
+
+const char* conv_tc_name(ConvTcPlan* cp) { return cp->name.c_str(); }
+
+template <typename T, int BN, bool RELU6>
+static int conv_launch_inst(ConvTcPlan* cp, cudaStream_t st) {
+    auto kern = conv_tc_kernel<T, BN, RELU6>;
+    static PerDeviceOnce attr_set;             // the opt-in is per device (and per kernel instance)
+    int dev = -1;
+    FD_CUDA_OK(cudaGetDevice(&dev));
+    if (attr_set.need(dev)) {
+        FD_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        attr_set.done(dev);
+    }
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = cp->grid; cfg.blockDim = dim3(CV_THREADS); cfg.dynamicSmemBytes = cp->smem_bytes; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = cp->opts.pdl ? 1 : 0;
+    FD_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, cp->tm_in, cp->tm_w, cp->tm_o[0], cp->tm_o[1], cp->tm_o[2], cp->tm_o[3], cp->p));
+    FD_CUDA_OK(cudaGetLastError());
+    return FD_OK;
+}
+
+template <typename T>
+static int conv_launch_t(ConvTcPlan* cp, cudaStream_t st) {
+    const bool r6 = cp->act == FD_ACT_RELU6;
+    switch (cp->po.bn) {
+        case 64: return r6 ? conv_launch_inst<T, 64, true>(cp, st) : conv_launch_inst<T, 64, false>(cp, st);
+        case 128: return r6 ? conv_launch_inst<T, 128, true>(cp, st) : conv_launch_inst<T, 128, false>(cp, st);
+        case 256: return r6 ? conv_launch_inst<T, 256, true>(cp, st) : conv_launch_inst<T, 256, false>(cp, st);
+        default: return fail(FD_ERR_UNSUPPORTED, "no conv_tc_kernel instance for this bn");
+    }
+}
+
+int conv_tc_launch(ConvTcPlan* cp, cudaStream_t st) {
+    return cp->dtype == FD_F16 ? conv_launch_t<__half>(cp, st) : conv_launch_t<__nv_bfloat16>(cp, st);
+}
+
+}  // namespace fd

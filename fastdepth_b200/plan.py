@@ -53,10 +53,10 @@ def _sq(v):
 
 
 def _blocks_of(module):
-    """(encoder blocks[14], decoder blocks[5], head, skips?) for the two module shapes on the hot path:
+    """(encoder blocks[14], decoder blocks[5], head, skips?) for the module shapes on the hot path:
     ``MobileNetSkipAdd`` (children conv0..13, decode_conv1..6; reference models.py:674-698) and
-    ``MobileNet`` with the depthwise NNConv decoder (children mobilenet[0..13], decoder.conv1..6; reference
-    models.py:229-244, 441-455)."""
+    ``MobileNet`` with an NNConv decoder, depthwise or dense (children mobilenet[0..13], decoder.conv1..6; reference
+    models.py:229-270, 441-455)."""
     if hasattr(module, 'conv0') and hasattr(module, 'decode_conv6'):
         enc = [getattr(module, 'conv%d' % i) for i in range(14)]
         dec = [getattr(module, 'decode_conv%d' % j) for j in range(1, 6)]
@@ -74,12 +74,29 @@ def _blocks_of(module):
     raise RuntimeError('unsupported module for the fastdepth_b200 hot path: %s' % type(module).__name__)
 
 
+def _is_dense_block(b):
+    """conv(C, C', k) of the dense NNConv decoder (reference models.py:52-59): Conv2d(groups 1, stride 1, k in {3, 5}),
+    BatchNorm2d, ReLU."""
+    return (isinstance(b, nn.Sequential) and len(b) == 3 and isinstance(b[0], nn.Conv2d) and b[0].groups == 1 and
+            _sq(b[0].kernel_size) in (3, 5) and _sq(b[0].stride) == 1 and isinstance(b[1], nn.BatchNorm2d))
+
+
+def dense_decoder(module):
+    """True if the module's decoder is the dense NNConv decoder (``MobileNet('nnconv5')`` / ``('nnconv3')``)."""
+    try:
+        _, dec, _, _, _ = _blocks_of(module)
+        return all(_is_dense_block(b) for b in dec)
+    except Exception:
+        return False
+
+
 def supports(module):
-    """True if ``describe`` can express the module: depthwise-separable decoder blocks of two Sequentials."""
+    """True if ``describe`` can express the module: depthwise-separable decoder blocks of two Sequentials, or dense
+    k x k conv blocks (k in {3, 5}) of the NNConv decoder."""
     try:
         enc, dec, head, _, _ = _blocks_of(module)
         return all(isinstance(b, nn.Sequential) and len(b) == 2 and isinstance(b[0], nn.Sequential) and
-                   b[0][0].groups == b[0][0].in_channels for b in dec)
+                   b[0][0].groups == b[0][0].in_channels for b in dec) or dense_decoder(module)
     except Exception:
         return False
 
@@ -89,7 +106,8 @@ def describe(module):
     tuples, stage names).
 
     Mirrors the dispatch of reference models.py:706-732 (SkipAdd: skips saved after encoder blocks 1/3/5 and added
-    after decoder stages 4/3/2) and models.py:253-270, 457-460 (MobileNet + NNConv: no skips)."""
+    after decoder stages 4/3/2) and models.py:253-270, 457-460 (MobileNet + NNConv: no skips; a dense decoder block
+    becomes one CONV stage with the weight tuple ``(None, None, None, w.reshape(c_out, -1), scale, bias)``)."""
     enc, dec, hd, with_skips, names = _blocks_of(module)
     descs, weights = [], []
     conv0 = enc[0]
@@ -113,6 +131,14 @@ def describe(module):
         stage_of_encoder[i] = len(descs) - 1
     for j in range(1, 6):
         blk = dec[j - 1]
+        if _is_dense_block(blk):
+            # dense kxk conv + BN + ReLU, then the nearest x2 upsample (reference models.py:52-59, 261-270)
+            c, bn, a = blk[0], blk[1], blk[2]
+            descs.append(dict(kind=_lib.FD_STAGE_CONV, c_in=c.weight.shape[1], c_out=c.weight.shape[0],
+                              ksize=_sq(c.kernel_size), stride=1, act=_act_of(a), upsample=1, skip_src=-1))
+            s, b = fold_bn(bn)
+            weights.append((None, None, None, _w(c).reshape(c.weight.shape[0], -1), s, b))
+            continue
         (dw, bn1, a1), (pw, bn2, a2) = (blk[0][0], blk[0][1], blk[0][2]), (blk[1][0], blk[1][1], blk[1][2])
         if _act_of(a1) != _act_of(a2):
             raise RuntimeError('decoder block %d: mixed activations are not supported' % j)

@@ -159,3 +159,60 @@ def to_mobilenet_keys(sd):
             i, rest = k[len('conv'):].split('.', 1)
             out['mobilenet.%s.%s' % (i, rest)] = v
     return out
+
+
+def synthetic_nnconv_state_dict(kernel_size=5, seed=1, calib_hw=(96, 128)):
+    """state_dict with the ``models.MobileNet('nnconv<k>')`` key schema (dense NNConv decoder, reference models.py:52-59,
+    245-270): the encoder of ``synthetic_state_dict(STOCK_WIDTHS, seed)`` (renamed with ``to_mobilenet_keys``), then five
+    dense ``conv(C, C/2, k)`` blocks and ``pointwise(32, 1)`` drawn from a separate seeded stream.
+
+    Same recipe as the depthwise decoder: conv weights U(-b, b) with b = 1/sqrt(fan_in) (fan_in = k*k*C), BN gamma / beta
+    drawn as above and running statistics CALIBRATED in fp64 on the encoder output of the same probe batch, a positive head
+    with gamma = 1, beta = 3.  Measured conditioning (storage-emulated forward against the fp32 forward, seed 1): fp16
+    2.5e-3 at 2x64x96 but 1.5e-2 at 1x224x224 (bf16 2.5e-2 / 1.2e-1); calibrating the decoder on a 224 x 224 probe instead
+    does not change that.  The functions above are untouched, so their fixtures stay bit-identical."""
+    import torch.nn.functional as F
+    base = to_mobilenet_keys(synthetic_state_dict(STOCK_WIDTHS, seed=seed, calib_hw=calib_hw))
+    sd = {k: v for k, v in base.items() if k.startswith('mobilenet.')}
+    f64 = torch.float64
+
+    def bn(t, prefix, hi):
+        g, b = sd[prefix + '.weight'].to(f64), sd[prefix + '.bias'].to(f64)
+        m, v = sd[prefix + '.running_mean'].to(f64), sd[prefix + '.running_var'].to(f64)
+        inv = g / torch.sqrt(v + 1e-5)
+        y = t * inv.view(1, -1, 1, 1) + (b - m * inv).view(1, -1, 1, 1)
+        return y.clamp(0.0, hi) if hi is not None else y.clamp_min(0.0)
+
+    strides = (2, 1, 2, 1, 2, 1, 2, 1, 1, 1, 1, 1, 2, 1)
+    x = torch.from_numpy(np.random.Generator(np.random.PCG64(seed + 7919)).random((2, 3) + tuple(calib_hw)))
+    x = bn(F.conv2d(x, sd['mobilenet.0.0.weight'].to(f64), None, 2, 1), 'mobilenet.0.1', 6.0)
+    for i in range(1, 14):
+        ci = sd['mobilenet.%d.0.weight' % i].shape[0]
+        x = bn(F.conv2d(x, sd['mobilenet.%d.0.weight' % i].to(f64), None, strides[i], 1, 1, ci), 'mobilenet.%d.1' % i, 6.0)
+        x = bn(F.conv2d(x, sd['mobilenet.%d.3.weight' % i].to(f64)), 'mobilenet.%d.4' % i, 6.0)
+    rng = np.random.Generator(np.random.PCG64(seed + 104729))
+    k, c = int(kernel_size), STOCK_ENCODER[13]
+
+    def calibrate(t, prefix, last=False):
+        ch = t.shape[1]
+        if last:
+            gamma, beta = np.ones(ch), np.full(ch, 3.0)
+        else:
+            gamma, beta = rng.uniform(GAMMA_RANGE[0], GAMMA_RANGE[1], ch), rng.normal(BETA[0], BETA[1], ch)
+        sd[prefix + '.weight'] = torch.from_numpy(gamma).float()
+        sd[prefix + '.bias'] = torch.from_numpy(beta).float()
+        sd[prefix + '.running_mean'] = t.mean(dim=(0, 2, 3)).float()
+        sd[prefix + '.running_var'] = t.var(dim=(0, 2, 3), unbiased=False).float()
+        sd[prefix + '.num_batches_tracked'] = torch.zeros((), dtype=torch.int64)
+        return bn(t, prefix, None)
+
+    for j, co in enumerate(STOCK_DECODER, start=1):
+        b = 1.0 / np.sqrt(k * k * c)
+        sd['decoder.conv%d.0.weight' % j] = torch.from_numpy(rng.uniform(-b, b, (co, c, k, k))).float().contiguous()
+        x = calibrate(F.conv2d(x, sd['decoder.conv%d.0.weight' % j].to(f64), None, 1, (k - 1) // 2), 'decoder.conv%d.1' % j)
+        x = x.repeat_interleave(2, dim=2).repeat_interleave(2, dim=3)
+        c = co
+    b = 1.0 / np.sqrt(c)
+    sd['decoder.conv6.0.weight'] = torch.from_numpy(np.abs(rng.uniform(-b, b, (1, c, 1, 1)))).float().contiguous()
+    calibrate(F.conv2d(x, sd['decoder.conv6.0.weight'].to(f64)), 'decoder.conv6.1', last=True)
+    return sd

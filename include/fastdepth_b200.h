@@ -55,8 +55,11 @@ typedef enum {
     FD_STAGE_DWPW = 1,   /* depthwise kxk(stride) + BN + act -> pointwise 1x1 + BN + act
                             (conv_dw, reference imagenet/mobilenet.py:29-38;
                              depthwise+pointwise, reference models.py:61-75, 683-697)        */
-    FD_STAGE_HEAD = 2    /* pointwise C->1 + BN + act, NHWC in -> [N,1,H,W] out
+    FD_STAGE_HEAD = 2,   /* pointwise C->1 + BN + act, NHWC in -> [N,1,H,W] out
                             (decode_conv6, reference models.py:698, 731)                     */
+    FD_STAGE_CONV = 3    /* dense kxk (k in {3,5}) stride-1 conv, padding (k-1)/2, + BN + act, then the
+                            optional nearest x2 upsample; NHWC in -> NHWC out.  No skip, no stride 2
+                            (conv() blocks of the dense NNConv decoder, reference models.py:52-59, 245-270) */
 } fd_stage_kind;
 
 typedef enum { FD_ACT_RELU = 0, FD_ACT_RELU6 = 1 } fd_act;
@@ -76,7 +79,7 @@ typedef struct {
                             models.py:806-811) -- the next stage then has c_in = c_out + c_skip  */
 } fd_stage_desc;
 
-/* Build a plan for a stage list (always: 1 STEM, k DWPW, 1 HEAD) at a fixed problem size.
+/* Build a plan for a stage list (always: 1 STEM, k stages each DWPW or CONV, 1 HEAD) at a fixed problem size.
  * Allocates NHWC activation buffers and packed-weight storage on `device`.
  * H and W must be multiples of 32 (reference forward's skip shapes only line up then),
  * every c_in/c_out except the stem's c_in and the head's c_out a multiple of 8. */
@@ -89,6 +92,8 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages,
  * parameter update.
  *   STEM : dw_* = NULL ; pw_w = [c_out][c_in][k][k]  ; pw_scale/pw_bias = [c_out]
  *   DWPW : dw_w = [c_in][k][k], dw_scale/dw_bias = [c_in] ; pw_w = [c_out][c_in], pw_scale/pw_bias = [c_out]
+ *   CONV : dw_* = NULL ; pw_w = [c_out][c_in][k][k]  ; pw_scale/pw_bias = [c_out]  (PyTorch's layout; the
+ *          plan keeps it as [c_out][k*k][c_in] in the plan dtype, the K-major operand both conv kernels read)
  *   HEAD : dw_* = NULL ; pw_w = [1][c_in]            ; pw_scale/pw_bias = [1]              */
 int fd_plan_set_stage_weights(fd_plan* plan, int stage,
                               const float* dw_w, const float* dw_scale, const float* dw_bias,
@@ -143,7 +148,7 @@ int fd_pipeline_wait(fd_plan* plan, unsigned long long ticket);
 /* Introspection for stage-parity tests: the NHWC buffer stage `stage` wrote in the last
  * fd_forward (valid until the next one).  c_stride = elements between pixels.
  * which = 0: the stage output (after upsample/skip-add); 1: the depthwise intermediate
- * (only materialised on path 0). */
+ * (only materialised on path 0; a CONV stage has none and fails with FD_ERR_INVALID). */
 int fd_stage_buffer(fd_plan* plan, int stage, int which, void** dev_ptr,
                     int* n, int* h, int* w, int* c, int* c_stride);
 
@@ -178,6 +183,12 @@ int fd_plan_trace_stage(fd_plan* plan, int stage, void* y_dev, void* stream,
  * in_stage_stride, cs (cluster size: CTAs sharing one tile's depthwise half), dw_teams}.  cap must be at least 16. */
 int fd_debug_block_plan(int ksize, int stride, int h_out, int w_out, int n, int c_in, int c_out, int head,
                         int* out, int cap);
+
+/* Debug (host only, needs no GPU): the tile plan of the dense conv kernel (conv_tc_kernel) for one CONV stage on
+ * `n_sms` SMs.  out[0..15] = {ok, ni, th, tw (tile = ni images x th rows x tw columns = 128 output pixels), bn (output
+ * channels per item), stages (operand ring depth), m_tiles, n_splits, items, waves, kblocks (64-channel blocks per
+ * tap), smem_bytes, useful_rows_permille, cost (modelled time, arbitrary units), 0, 0}.  cap must be at least 16. */
+int fd_debug_conv_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms, int* out, int cap);
 
 /* Per-image depth metrics on device (reference metrics.py:31-55 applied per image, as
  * main.py:40-41,80-82 does at batch size 1).  pred: [n, hw] of `dtype`; target: [n, hw] fp32.

@@ -17,10 +17,14 @@ What is here and what is not (SURVEY.md section 2 / section 8):
   ``fastdepth_b200`` plan and makes one C-ABI call.  There is NO CPU fallback
   and NO PyTorch-eager fallback: a missing extension or a CPU tensor raises.
 * ``MobileNet`` + ``NNConv``  -- BASELINE config 1 plumbing
-  ("MobileNet-NNConv5", dense or depthwise decoder, no skips).  On CPU, and with
-  the dense 5x5 decoder everywhere, it is plain PyTorch exactly like the reference;
-  a CUDA tensor through the depthwise decoder ("MobileNet-NNConv5(depthwise)",
-  SURVEY.md section 8f row 2) takes the same fused kernels as MobileNetSkipAdd.
+  ("MobileNet-NNConv5", dense or depthwise decoder, no skips).  On CPU it is plain
+  PyTorch exactly like the reference.  A CUDA tensor through the depthwise decoder
+  ("MobileNet-NNConv5(depthwise)", SURVEY.md section 8f row 2) takes the same fused
+  kernels as MobileNetSkipAdd; an fp16 / bf16 CUDA tensor through the dense decoder
+  ("MobileNet-NNConv5") runs the encoder on those kernels and every dense 5x5 decoder
+  conv on the implicit-GEMM wgmma kernel (fd_conv_tc.cu).  The dense decoder in fp32
+  stays on stock PyTorch: the project's fp32 path is SIMT, while cuDNN may run fp32
+  convolutions on TF32 tensor cores (tools/bench_nnconv5.py measures both).
 * every other decoder/encoder family of the reference (DeConv, UpConv, UpProj,
   BLConv, ShuffleConv, ResNet*) is out of scope of this tier; ``choose_decoder``
   names them in its error.
@@ -170,14 +174,16 @@ class MobileNet(nn.Module):
         return state
 
     def forward(self, x):
-        """CPU tensors (BASELINE config 1 plumbing) and the dense 5x5 decoder run on stock PyTorch, exactly like the
-        reference (models.py:457-460).  A CUDA tensor through the depthwise NNConv decoder ("MobileNet-NNConv5(dw)",
-        reference README.md:37) takes the same fused sm_90a path as MobileNetSkipAdd, just without skips."""
+        """CPU tensors (BASELINE config 1 plumbing) run on stock PyTorch, exactly like the reference (models.py:457-460).
+        A CUDA tensor through the depthwise NNConv decoder ("MobileNet-NNConv5(dw)", reference README.md:37) takes the same
+        fused sm_90a path as MobileNetSkipAdd, just without skips.  A CUDA fp16 / bf16 tensor through the dense decoder
+        ("MobileNet-NNConv5", README.md:36) takes the engine too, with the decoder convs on conv_tc_kernel; the dense
+        decoder in fp32 stays on stock PyTorch (cuDNN may use TF32 tensor cores there, the project's fp32 path is SIMT)."""
         fused_ok = (x.is_cuda and not self.training and x.dim() == 4 and x.shape[1] == 3 and
                     x.shape[2] % 32 == 0 and x.shape[3] % 32 == 0)     # what the fused plan covers; anything else: stock PyTorch
         if fused_ok:
             from fastdepth_b200 import plan as _plan
-            if _plan.supports(self):
+            if _plan.supports(self) and not (x.dtype == torch.float32 and _plan.dense_decoder(self)):
                 engine = self.__dict__.get('_fd_engine')
                 if engine is None:
                     from fastdepth_b200.engine import SkipAddEngine
