@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('FD_B200_LIB') or os.path.join(HERE, 'libfastdepth_b200.so')   # env: developer A/B of kernel variants
 
 FD_F32, FD_F16, FD_BF16 = 0, 1, 2
-FD_STAGE_STEM, FD_STAGE_DWPW, FD_STAGE_HEAD, FD_STAGE_CONV = 0, 1, 2, 3
+FD_STAGE_STEM, FD_STAGE_DWPW, FD_STAGE_HEAD, FD_STAGE_CONV, FD_STAGE_DECONV, FD_STAGE_UPCONV = 0, 1, 2, 3, 4, 5
 FD_ACT_RELU, FD_ACT_RELU6 = 0, 1
 
 
@@ -52,6 +52,7 @@ SIGNATURES = {
                                            _c_int_p, _c_int_p]),
     'fd_debug_block_plan': (ctypes.c_int, [ctypes.c_int] * 8 + [_c_int_p, ctypes.c_int]),
     'fd_debug_conv_plan': (ctypes.c_int, [ctypes.c_int] * 7 + [_c_int_p, ctypes.c_int]),
+    'fd_debug_convt_plan': (ctypes.c_int, [ctypes.c_int] * 8 + [_c_int_p, ctypes.c_int]),
     'fd_metrics_accumulate': (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp,
                                              ctypes.c_int, _vp]),
     'fd_nyu_val_gather': (ctypes.c_int, [_vp, _vp, _vp, _vp] + [ctypes.c_int] * 6 + [_vp, _vp, ctypes.c_int, _vp]),

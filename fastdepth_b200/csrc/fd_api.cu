@@ -13,7 +13,7 @@
 namespace fd {
 
 BlockPlanOut block_tc_debug_plan(int ksize, int stride, int h_out, int w_out, int n, int c_in, int c_out, int head);
-ConvPlanOut conv_tc_debug_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms);
+ConvPlanOut conv_tc_debug_plan(int kind, int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms);
 
 // ---- error state -----------------------------------------------------------------------
 static thread_local std::string g_last_error;
@@ -30,6 +30,8 @@ int launch_dw(int dtype, const BlockArgs& a, cudaStream_t st);
 int launch_pw(int dtype, const BlockArgs& a, cudaStream_t st);
 int launch_conv(int dtype, const void* in, const void* w, void* out, const float* scale, const float* bias, const StageGeom& g,
                 cudaStream_t st);
+int launch_convt(int dtype, int kind, const void* in, const void* w, void* out, const float* scale, const float* bias,
+                 const StageGeom& g, cudaStream_t st);
 int launch_head(int dtype, const void* in, void* out, const float* w, float scale, float bias, long long m_total, int c,
                 int in_pitch, int h, int wd, int up, int act, cudaStream_t st);
 int launch_metrics(int dtype, const void* pred, const float* target, int n, int hw, double* sums, cudaStream_t st);
@@ -62,14 +64,16 @@ void stem_tc_destroy(StemTcPlan* sp);
 const char* stem_tc_name(StemTcPlan* sp);
 // dense kxk conv on wgmma (fd_conv_tc.cu)
 struct ConvTcPlan;
-bool conv_tc_supported(int dtype, const StageGeom& g);
-int conv_tc_prepare(int dtype, const StageGeom& g, const void* in, const void* w, const float* scale_dev, const float* bias_dev,
-                    void* out, const TcLaunchOpts& opts, ConvTcPlan** res);
+bool conv_tc_supported(int dtype, const StageGeom& g, int kind);
+int conv_tc_prepare(int dtype, int kind, const StageGeom& g, const void* in, const void* w, const float* scale_dev,
+                    const float* bias_dev, void* out, const TcLaunchOpts& opts, ConvTcPlan** res);
 int conv_tc_launch(ConvTcPlan* cp, cudaStream_t st);
 void conv_tc_destroy(ConvTcPlan* cp);
 const char* conv_tc_name(ConvTcPlan* cp);
 
 static size_t dtype_size(int dtype) { return dtype == FD_F32 ? 4 : 2; }
+static bool is_phased(int kind) { return kind == FD_STAGE_DECONV || kind == FD_STAGE_UPCONV; }
+static bool is_conv(int kind) { return kind == FD_STAGE_CONV || is_phased(kind); }
 
 struct Stage {
     fd_stage_desc d{};
@@ -85,7 +89,7 @@ struct Stage {
     float* dw_w = nullptr;               // [k*k][c_in]
     float* dw_scale = nullptr;
     float* dw_bias = nullptr;
-    void* pw_w = nullptr;                // [c_out][c_in] plan dtype (DWPW); [c_out][k*k][c_in] plan dtype (CONV)
+    void* pw_w = nullptr;                // [c_out][c_in] plan dtype (DWPW); [c_out][k*k][c_in] plan dtype (CONV, DECONV, UPCONV)
     float* pw_w_f32 = nullptr;           // stem: [27][c_out] tap-major ; head: [c_in]
     float* pw_scale = nullptr;
     float* pw_bias = nullptr;
@@ -238,33 +242,44 @@ static int build_steps(fd_plan* p) {
                 };
             }
             p->steps.push_back(st);
-        } else if (s.d.kind == FD_STAGE_CONV) {
+        } else if (is_conv(s.d.kind)) {
             // dense kxk conv: one implicit-GEMM step (path 1: conv_tc_kernel, else the SIMT conv_kernel); with the head folded
-            // below the last upsample the stage stores at conv resolution and head_kernel<up2x> replicates
+            // below the last upsample the stage stores at conv resolution and head_kernel<up2x> replicates.  DECONV / UPCONV:
+            // the same step as four phase convs at the input resolution (g.h_out == g.h_in), k*k*c_in*c_out MACs per input
+            // pixel, the 2h x 2w output written once (path 0: convt_kernel)
             StageGeom g = s.g;
             if (fold && &s == &last) g.upsample = 0;
+            const int kind = s.d.kind;
             const double px_in = (double)g.n * g.h_in * g.w_in, px_out = (double)g.n * g.h_out * g.w_out;
             const double kk = (double)g.ksize * g.ksize;
             Step st;
             st.stage = i;
             st.macs = px_out * g.c_in * g.c_out * kk;
             st.dw_macs = 0.0;
-            st.alg_bytes = (px_in * g.c_in + px_out * (g.upsample ? 4.0 : 1.0) * g.c_out) * es + kk * g.c_in * g.c_out * es +
-                           2.0 * g.c_out * 4;
+            st.alg_bytes = (px_in * g.c_in + px_out * (g.upsample || is_phased(kind) ? 4.0 : 1.0) * g.c_out) * es +
+                           kk * g.c_in * g.c_out * es + 2.0 * g.c_out * 4;
             const int dtype = p->dtype;
-            if (p->opt_path == 1 && conv_tc_supported(dtype, g)) {
-                int rc = conv_tc_prepare(dtype, g, in, s.pw_w, s.pw_scale, s.pw_bias, s.out, lopts, &s.ctc);
+            if (p->opt_path == 1 && conv_tc_supported(dtype, g, kind)) {
+                int rc = conv_tc_prepare(dtype, kind, g, in, s.pw_w, s.pw_scale, s.pw_bias, s.out, lopts, &s.ctc);
                 if (rc != FD_OK) return rc;
                 st.name = conv_tc_name(s.ctc);
                 ConvTcPlan* ctc = s.ctc;
                 st.run = [ctc](cudaStream_t stream, const void*, void*) { return conv_tc_launch(ctc, stream); };
-            } else {
+            } else if (kind == FD_STAGE_CONV) {
                 char nm[64];
                 snprintf(nm, sizeof(nm), "conv_kernel<k%d>", g.ksize);
                 st.name = nm;
                 Stage* sp = &s;
                 st.run = [sp, in, g, dtype](cudaStream_t stream, const void*, void*) {
                     return launch_conv(dtype, in, sp->pw_w, sp->out, sp->pw_scale, sp->pw_bias, g, stream);
+                };
+            } else {
+                char nm[64];
+                snprintf(nm, sizeof(nm), "convt_kernel<%s%d>", kind == FD_STAGE_DECONV ? "deconv" : "upconv", g.ksize);
+                st.name = nm;
+                Stage* sp = &s;
+                st.run = [sp, in, g, dtype, kind](cudaStream_t stream, const void*, void*) {
+                    return launch_convt(dtype, kind, in, sp->pw_w, sp->out, sp->pw_scale, sp->pw_bias, g, stream);
                 };
             }
             p->steps.push_back(st);
@@ -449,8 +464,8 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages, int n, int h, int 
         const fd_stage_desc& d = s.d;
         const bool first = i == 0, lastst = i == n_stages - 1;
         if ((d.kind == FD_STAGE_STEM) != first || (d.kind == FD_STAGE_HEAD) != lastst ||
-            (!first && !lastst && d.kind != FD_STAGE_DWPW && d.kind != FD_STAGE_CONV)) {
-            rc = fail(FD_ERR_INVALID, "stage list must be STEM, (DWPW|CONV)..., HEAD"); break; }
+            (!first && !lastst && d.kind != FD_STAGE_DWPW && !is_conv(d.kind))) {
+            rc = fail(FD_ERR_INVALID, "stage list must be STEM, (DWPW|CONV|DECONV|UPCONV)..., HEAD"); break; }
         if (d.c_in != ch) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": c_in does not match producer"); break; }
         if (d.act != FD_ACT_RELU && d.act != FD_ACT_RELU6) { rc = fail(FD_ERR_INVALID, "bad act"); break; }
         s.g.n = n; s.g.h_in = hh; s.g.w_in = ww; s.g.c_in = d.c_in; s.g.c_out = d.c_out;
@@ -470,13 +485,24 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages, int n, int h, int 
             if ((d.ksize != 3 && d.ksize != 5) || d.c_in % 8 || d.c_out % 8 || d.c_out <= 0 || (d.upsample != 0 && d.upsample != 1)) {
                 rc = fail(FD_ERR_INVALID, "conv stage needs k in {3,5}, channels % 8 == 0, upsample 0|1"); break; }
             s.g.h_out = hh; s.g.w_out = ww;
+        } else if (is_phased(d.kind)) {
+            const char* nm = d.kind == FD_STAGE_DECONV ? "a DECONV" : "an UPCONV";
+            if (d.skip_src >= 0) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": " + nm + " stage takes no skip"); break; }
+            if (d.stride != 2) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": " + nm + " stage has stride 2"); break; }
+            if (d.upsample != 0) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": " + nm + " stage has upsample 0"); break; }
+            const bool k_ok = d.kind == FD_STAGE_DECONV ? (d.ksize == 3 || d.ksize == 5 || d.ksize == 7 || d.ksize == 9) : d.ksize == 5;
+            if (!k_ok || d.c_in % 8 || d.c_out % 8 || d.c_out <= 0) {
+                rc = fail(FD_ERR_INVALID, d.kind == FD_STAGE_DECONV ? "deconv stage needs k in {3,5,7,9}, channels % 8 == 0"
+                                                                    : "upconv stage needs k 5, channels % 8 == 0");
+                break; }
+            s.g.h_out = hh; s.g.w_out = ww;            // the phase convs run at the input resolution; the output is 2h x 2w
         } else {
             if (d.ksize != 1 || d.c_out != 1 || d.c_in % 8 || d.upsample || d.skip_src >= 0) {
                 rc = fail(FD_ERR_INVALID, "head must be 1x1, c_out 1, c_in % 8 == 0"); break; }
             s.g.h_out = hh; s.g.w_out = ww;
         }
-        s.out_h = s.g.h_out * (s.g.upsample ? 2 : 1);
-        s.out_w = s.g.w_out * (s.g.upsample ? 2 : 1);
+        s.out_h = s.g.h_out * (s.g.upsample || is_phased(d.kind) ? 2 : 1);
+        s.out_w = s.g.w_out * (s.g.upsample || is_phased(d.kind) ? 2 : 1);
         s.out_c = d.c_out; s.out_pitch = d.c_out;
         if (d.skip_src >= 0) {
             if (d.kind != FD_STAGE_DWPW || !d.upsample || d.skip_src >= i) { rc = fail(FD_ERR_INVALID, "bad skip_src"); break; }
@@ -509,7 +535,7 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages, int n, int h, int 
             if ((rc = dev_alloc(p, (void**)&s.dw_scale, (size_t)d.c_in * 4))) break;
             if ((rc = dev_alloc(p, (void**)&s.dw_bias, (size_t)d.c_in * 4))) break;
             if ((rc = dev_alloc(p, &s.pw_w, (size_t)d.c_in * d.c_out * es))) break;
-        } else if (d.kind == FD_STAGE_CONV) {
+        } else if (is_conv(d.kind)) {
             if ((rc = dev_alloc(p, &s.pw_w, (size_t)d.ksize * d.ksize * d.c_in * d.c_out * es))) break;
         } else if (d.kind == FD_STAGE_STEM) {
             if ((rc = dev_alloc(p, (void**)&s.pw_w_f32, (size_t)27 * d.c_out * 4))) break;
@@ -556,6 +582,26 @@ int fd_plan_set_stage_weights(fd_plan* p, int stage, const float* dw_w, const fl
         for (int co = 0; co < d.c_out; ++co)
             for (int ci = 0; ci < d.c_in; ++ci)
                 for (int j = 0; j < kk; ++j) t[((size_t)co * kk + j) * d.c_in + ci] = pw_w[((size_t)co * d.c_in + ci) * kk + j];
+        int rc = upload_as_dtype(p->dtype, t.data(), t.size(), s.pw_w);
+        if (rc) return rc;
+    } else if (is_phased(d.kind)) {
+        // DECONV [ci][co][ty][tx] / UPCONV [co][ci][ty][tx] -> [co][phase-major taps][ci]: phase q = 2 ry + rx holds its taps
+        // sorted by (dy, dx), weight tap (convt_tap(ry, dy), convt_tap(rx, dx)) (fd_conv_plan.h)
+        const int k = d.ksize, kk = k * k;
+        ConvPhase ph[4];
+        conv_phases(d.kind, k, ph);
+        std::vector<float> t((size_t)d.c_out * kk * d.c_in);
+        for (int q = 0; q < 4; ++q)
+            for (int iy = 0; iy < ph[q].ny; ++iy)
+                for (int ix = 0; ix < ph[q].nx; ++ix) {
+                    const int tap = ph[q].tap0 + iy * ph[q].nx + ix;
+                    const int wy = convt_tap(d.kind, k, q >> 1, ph[q].dy0 + iy), wx = convt_tap(d.kind, k, q & 1, ph[q].dx0 + ix);
+                    for (int co = 0; co < d.c_out; ++co)
+                        for (int ci = 0; ci < d.c_in; ++ci) {
+                            const size_t src = d.kind == FD_STAGE_DECONV ? ((size_t)ci * d.c_out + co) * kk : ((size_t)co * d.c_in + ci) * kk;
+                            t[((size_t)co * kk + tap) * d.c_in + ci] = pw_w[src + wy * k + wx];
+                        }
+                }
         int rc = upload_as_dtype(p->dtype, t.data(), t.size(), s.pw_w);
         if (rc) return rc;
     } else if (d.kind == FD_STAGE_STEM) {
@@ -765,7 +811,7 @@ int fd_stage_buffer(fd_plan* p, int stage, int which, void** dev_ptr, int* n, in
         // with decode_conv6 folded below the last upsample the last block writes its low-res output
         if (p->opt_fold_head && stage == (int)p->stages.size() - 2 && s.d.upsample && s.d.skip_src < 0) { hh = s.g.h_out; ww = s.g.w_out; }
     } else if (which == 1) {
-        if (s.d.kind == FD_STAGE_CONV) return fail(FD_ERR_INVALID, "a CONV stage has no depthwise intermediate");
+        if (is_conv(s.d.kind)) return fail(FD_ERR_INVALID, "a CONV / DECONV / UPCONV stage has no depthwise intermediate");
         ptr = s.mid; hh = s.g.h_out; ww = s.g.w_out; cc = s.g.c_in;
     } else {
         return fail(FD_ERR_INVALID, "which must be 0 or 1");
@@ -869,7 +915,7 @@ int fd_plan_trace_stage(fd_plan* p, int stage, void* y_dev, void* stream, unsign
     int rc = ensure_steps(p);
     if (rc) return rc;
     if (cap < 12 * 256) return fail(FD_ERR_INVALID, "trace buffer too small (need 3072 entries)");
-    if (p->stages[stage].d.kind == FD_STAGE_CONV) return fail(FD_ERR_INVALID, "the stage timeline exists for fused block kernels only");
+    if (is_conv(p->stages[stage].d.kind)) return fail(FD_ERR_INVALID, "the stage timeline exists for fused block kernels only");
     if (p->stages[stage].chain) return chain_tc_trace(p->stages[stage].chain, (cudaStream_t)stream, out_host, rows, cols);
     if (!p->stages[stage].tc) return fail(FD_ERR_STATE, "stage does not run the fused block kernel");
     return block_tc_trace(p->stages[stage].tc, (cudaStream_t)stream, y_dev, out_host, rows, cols);
@@ -886,10 +932,26 @@ int fd_debug_block_plan(int ksize, int stride, int h_out, int w_out, int n, int 
 
 int fd_debug_conv_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms, int* out, int cap) {
     if (!out || cap < 16) return fail(FD_ERR_INVALID, "need an int[16] output");
-    const ConvPlanOut q = conv_tc_debug_plan(ksize, h_out, w_out, n, c_in, c_out, n_sms);
+    const ConvPlanOut q = conv_tc_debug_plan(FD_STAGE_CONV, ksize, h_out, w_out, n, c_in, c_out, n_sms);
     const int v[16] = {q.ok, q.ni, q.th, q.tw, q.bn, q.stages, q.m_tiles, q.n_splits, q.items, q.waves, q.kblocks, q.smem_bytes,
                        q.useful_permille, (int)(q.cost > 2e9 ? 2e9 : q.cost), 0, 0};
     for (int i = 0; i < 16; ++i) out[i] = v[i];
+    return FD_OK;
+}
+
+int fd_debug_convt_plan(int kind, int ksize, int h_in, int w_in, int n, int c_in, int c_out, int n_sms, int* out, int cap) {
+    if (!out || cap < 44) return fail(FD_ERR_INVALID, "need an int[44] output");
+    if (!is_phased(kind)) return fail(FD_ERR_INVALID, "kind must be FD_STAGE_DECONV or FD_STAGE_UPCONV");
+    const ConvPlanOut q = conv_tc_debug_plan(kind, ksize, h_in, w_in, n, c_in, c_out, n_sms);
+    const int v[16] = {q.ok, q.ni, q.th, q.tw, q.bn, q.stages, q.m_tiles, q.n_splits, q.items, q.waves, q.kblocks, q.smem_bytes,
+                       q.useful_permille, (int)(q.cost > 2e9 ? 2e9 : q.cost), q.groups, 0};
+    for (int i = 0; i < 16; ++i) out[i] = v[i];
+    for (int ph = 0; ph < 4; ++ph) {
+        const int e[5] = {q.ph[ph].tap0, q.ph[ph].ny, q.ph[ph].nx, q.ph[ph].dy0, q.ph[ph].dx0};
+        for (int j = 0; j < 5; ++j) out[16 + 5 * ph + j] = q.ok ? e[j] : 0;
+    }
+    for (int g = 0; g < 4; ++g)
+        for (int j = 0; j < 2; ++j) out[36 + 2 * g + j] = q.ok ? q.group_ph[g][j] : -1;
     return FD_OK;
 }
 

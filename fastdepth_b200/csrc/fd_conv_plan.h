@@ -9,6 +9,12 @@
 //     the shared-memory reads of the wgmma operands (both warpgroups read their A half and all of B) and the L2 -> SMEM
 //     operand traffic (16 KB of A + bn x 128 B of B) at an ESTIMATED 40 B / clock / SM (not measured);
 //   * the epilogue: the 16-bit output tile (x4 with the nearest upsample) leaves at an estimated 64 B / clock.
+//
+// Transposed conv (DECONV) and unpool + conv (UPCONV) stages are four stride-1 convs at the input resolution, one per output
+// parity (ry, rx): phase 2 ry + rx reads input (Y + dy, X + dx) for a box of (dy, dx) offsets with its own weight taps.  Phases
+// differ in cost (9 / 6 / 6 / 4 taps for k = 5), so an item is (tile, bn split, phase group): either one phase per item or the
+// two diagonal pairs {00, 11} and {01, 10}.  Items are ordered group-major, heaviest group first, and the cost model takes the
+// makespan of the persistent grid's static round-robin assignment over the real per-item tap counts.
 #pragma once
 
 namespace fd {
@@ -19,11 +25,55 @@ constexpr int kConvSmemBudget = 227 * 1024 - 128;
 constexpr int kConvAlignSlack = 1024;
 constexpr int kConvBarrierBytes = 256;                // >= sizeof(ConvBarriers)
 
+// stage kinds of the conv kernel (the fd_stage_kind values)
+constexpr int kConvKindConv = 3, kConvKindDeconv = 4, kConvKindUpconv = 5;
+
+// one phase of a conv: taps [tap0, tap0 + ny * nx) of the repacked weights [c_out][taps][c_in], tap tap0 + iy * nx + ix reads
+// input (Y + dy0 + iy, X + dx0 + ix) for conv-resolution pixel (Y, X)
+struct ConvPhase { int tap0, ny, nx, dy0, dx0; };
+
+// weight tap t (per axis, 0..k-1) of output parity r at input offset d; p = (k - 1) / 2.
+//   DECONV (ConvTranspose2d(k, 2, p, 1), weights [c_in][c_out][k][k], no flip): t = r + p - 2 d
+//   UPCONV (zero-insert x2, then Conv2d(k, 1, p), weights [c_out][c_in][k][k]): t = 2 d + p - r
+inline int convt_tap(int kind, int k, int r, int d) {
+    const int p = (k - 1) / 2;
+    return kind == kConvKindDeconv ? r + p - 2 * d : 2 * d + p - r;
+}
+
+// the contiguous range [d0, d0 + n) of input offsets of parity r (the taps with t = r + p mod 2)
+inline void convt_axis(int kind, int k, int r, int* d0, int* n) {
+    const int p = (k - 1) / 2;
+    int lo = 1 << 20, hi = -(1 << 20);
+    for (int t = 0; t < k; ++t) {
+        if ((t - r - p) & 1) continue;
+        const int d = kind == kConvKindDeconv ? (r + p - t) / 2 : (r + t - p) / 2;
+        lo = d < lo ? d : lo; hi = d > hi ? d : hi;
+    }
+    *d0 = lo; *n = hi - lo + 1;
+}
+
+// the phase table of a stage: CONV is one phase, the k x k square in (ky, kx) order; DECONV / UPCONV are four, phase
+// 2 ry + rx, their taps stored phase-major and sorted by (dy, dx).  Returns the number of phases.
+inline int conv_phases(int kind, int k, ConvPhase ph[4]) {
+    const int p = (k - 1) / 2;
+    if (kind == kConvKindConv) { ph[0] = ConvPhase{0, k, k, -p, -p}; return 1; }
+    int tap0 = 0;
+    for (int q = 0; q < 4; ++q) {
+        convt_axis(kind, k, q >> 1, &ph[q].dy0, &ph[q].ny);
+        convt_axis(kind, k, q & 1, &ph[q].dx0, &ph[q].nx);
+        ph[q].tap0 = tap0;
+        tap0 += ph[q].ny * ph[q].nx;
+    }
+    return 4;
+}
+
 struct ConvPlanIn {
-    int ksize, h_out, w_out, n, c_in, c_out, upsample;
+    int ksize, h_out, w_out, n, c_in, c_out, upsample;   // h_out / w_out: the conv resolution (a DECONV's input map)
     int n_sms;                 // 0 = 132 (H100 SXM)
     int force_bn;              // 0 = the cost model chooses, else 64 / 128 / 256
     int force_tile;            // -1 = the cost model chooses, else an index into kConvTiles
+    int kind;                  // kConvKind*; 0 = CONV
+    int force_group;           // phases per item of a DECONV / UPCONV stage: 0 = the cost model chooses, 1 = one, 2 = pairs
 };
 struct ConvPlanOut {
     int ok;
@@ -31,6 +81,9 @@ struct ConvPlanOut {
     int m_tiles, n_splits, items, waves, kblocks;
     int smem_bytes, useful_permille;
     double cost;
+    int n_phases, groups;       // items = m_tiles * n_splits * groups
+    ConvPhase ph[4];
+    int group_ph[4][2];         // phases of group g, in order; -1 = none
 };
 
 // candidate tiles (images x rows x columns, 128 pixels each); small maps take several images per box
@@ -39,15 +92,34 @@ constexpr int kConvNumTiles = 5;
 
 inline int conv_stage_bytes(int bn) { return 128 * 128 + bn * 128; }
 
-inline ConvPlanOut plan_conv_one(const ConvPlanIn& q, int tile, int bn) {
+inline ConvPlanOut plan_conv_one(const ConvPlanIn& q, int tile, int bn, int per_item) {
     ConvPlanOut o{};
+    const int kind = q.kind ? q.kind : kConvKindConv;
+    o.n_phases = conv_phases(kind, q.ksize, o.ph);
+    for (int g = 0; g < 4; ++g) o.group_ph[g][0] = o.group_ph[g][1] = -1;
+    if (o.n_phases == 1) {
+        o.groups = 1; o.group_ph[0][0] = 0;
+    } else if (per_item == 2) {                     // the diagonal pairs, the heavier pair first
+        const int t03 = o.ph[0].ny * o.ph[0].nx + o.ph[3].ny * o.ph[3].nx, t12 = o.ph[1].ny * o.ph[1].nx + o.ph[2].ny * o.ph[2].nx;
+        o.groups = 2;
+        o.group_ph[t03 >= t12 ? 0 : 1][0] = 0; o.group_ph[t03 >= t12 ? 0 : 1][1] = 3;
+        o.group_ph[t03 >= t12 ? 1 : 0][0] = 1; o.group_ph[t03 >= t12 ? 1 : 0][1] = 2;
+    } else {                                        // one phase per item, heaviest first (stable)
+        o.groups = 4;
+        int order[4] = {0, 1, 2, 3};
+        for (int a = 1; a < 4; ++a)
+            for (int b = a; b > 0 && o.ph[order[b]].ny * o.ph[order[b]].nx > o.ph[order[b - 1]].ny * o.ph[order[b - 1]].nx; --b) {
+                const int t = order[b]; order[b] = order[b - 1]; order[b - 1] = t;
+            }
+        for (int g = 0; g < 4; ++g) o.group_ph[g][0] = order[g];
+    }
     const int ni = kConvTiles[tile][0], th = kConvTiles[tile][1], tw = kConvTiles[tile][2];
     const int sms = q.n_sms > 0 ? q.n_sms : 132;
     o.ni = ni; o.th = th; o.tw = tw; o.bn = bn;
     o.kblocks = (q.c_in + 63) / 64;
     o.m_tiles = ((q.n + ni - 1) / ni) * ((q.h_out + th - 1) / th) * ((q.w_out + tw - 1) / tw);
     o.n_splits = (q.c_out + bn - 1) / bn;
-    o.items = o.m_tiles * o.n_splits;
+    o.items = o.m_tiles * o.n_splits * o.groups;
     o.waves = (o.items + sms - 1) / sms;
     const int fixed = 2 * kConvStg + kConvBarrierBytes + kConvAlignSlack;
     o.stages = (kConvSmemBudget - fixed) / conv_stage_bytes(bn);
@@ -62,15 +134,34 @@ inline ConvPlanOut plan_conv_one(const ConvPlanIn& q, int tile, int bn) {
     if (smem_rd > kstep) kstep = smem_rd;
     if (l2 > kstep) kstep = l2;
     kstep += 40.0;                                    // barrier hand-shakes per K-block
-    const double steps = (double)q.ksize * q.ksize * o.kblocks;
     const double epi = 128.0 * bn * 2.0 * (q.upsample ? 4.0 : 1.0) / 64.0 + 500.0;
-    o.cost = (double)o.waves * (steps * kstep + epi);
+    // makespan of the static round-robin: CTA b of G runs items b, b + G, ...; group g holds items [g * per, (g + 1) * per)
+    const int G = o.items < sms ? o.items : sms, per = o.m_tiles * o.n_splits;
+    double gcost[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int g = 0; g < o.groups; ++g)
+        for (int j = 0; j < 2; ++j) {
+            const int ph = o.group_ph[g][j];
+            if (ph >= 0) gcost[g] += (double)o.ph[ph].ny * o.ph[ph].nx * o.kblocks * kstep + epi;
+        }
+    auto fdiv = [](long long a, long long b) { return a >= 0 ? a / b : -((-a + b - 1) / b); };
+    o.cost = 0.0;
+    for (int b = 0; b < G && G > 0; ++b) {
+        double c = 0.0;
+        for (int g = 0; g < o.groups; ++g) {
+            const long long s0 = (long long)g * per, s1 = s0 + per;          // items w in [s0, s1) with w % G == b
+            c += gcost[g] * (double)(fdiv(s1 - 1 - b, G) - fdiv(s0 - 1 - b, G));
+        }
+        if (c > o.cost) o.cost = c;
+    }
     return o;
 }
 
 inline ConvPlanOut plan_conv(const ConvPlanIn& q) {
     ConvPlanOut best{};
     best.ok = 0;
+    const bool phased = q.kind == kConvKindDeconv || q.kind == kConvKindUpconv;
+    if (q.force_group && (!phased || q.force_group > 2)) return best;
+    if (phased && (q.ksize < 3 || q.ksize > 9 || !(q.ksize & 1))) return best;
     if (q.ksize < 1 || q.h_out < 1 || q.w_out < 1 || q.n < 1 || q.c_in < 8 || q.c_out < 8) return best;
     const int bns[3] = {64, 128, 256};
     for (int t = 0; t < kConvNumTiles; ++t) {
@@ -78,9 +169,13 @@ inline ConvPlanOut plan_conv(const ConvPlanIn& q) {
         for (int b = 0; b < 3; ++b) {
             const int bn = bns[b];
             if (q.force_bn ? bn != q.force_bn : (b > 0 && bn / 2 >= q.c_out)) continue;   // no split wider than twice the need
-            const ConvPlanOut o = plan_conv_one(q, t, bn);
-            if (!o.ok) continue;
-            if (!best.ok || o.cost < best.cost * 0.999) best = o;   // ties keep the earlier (larger-row, narrower) choice
+            for (int per_item = 1; per_item <= 2; ++per_item) {
+                if (q.force_group ? per_item != q.force_group : (per_item == 2 && (q.kind == 0 || q.kind == kConvKindConv)))
+                    continue;
+                const ConvPlanOut o = plan_conv_one(q, t, bn, per_item);
+                if (!o.ok) continue;
+                if (!best.ok || o.cost < best.cost * 0.999) best = o;   // ties keep the earlier (larger-row, narrower) choice
+            }
         }
     }
     return best;

@@ -13,6 +13,11 @@
 //                             register accumulators, one commit group kept in flight; then BN affine + act -> 16-bit -> staging
 //                             tile -> TMA tensor stores (four strided views of the output for the nearest x2 upsample)
 // One mbarrier ring of operand stages (A + B) between the producer and the consumers.
+//
+// The same kernel runs the transposed conv (DECONV) and unpool + conv (UPCONV) stages as four stride-1 phase convs at the
+// input resolution (fd_conv_plan.h): an item is then (tile, bn split, phase group); the producer's box loop and the
+// consumers' K loop come from the phase's {tap0, ny, nx, dy0, dx0}, and phase 2 ry + rx is stored through output view
+// tm_o[2 ry + rx] (the same four strided views as the upsample).  A CONV stage is one phase, the k x k square.
 #include <cstdio>
 #include <cstring>
 #include <new>
@@ -29,11 +34,14 @@ constexpr int CV_A_BYTES = 128 * 128;
 struct ConvParams {
     int n, h, w, c_in, c_out;        // conv input == conv output size (stride 1, same padding)
     int ni, th, tw;                  // tile: ni images x th rows x tw columns = 128 pixels
-    int tiles_x, tiles_y, splits, items;
-    int ks, pad, kblocks, ksteps;    // ksteps = ks * ks * kblocks
+    int tiles_x, tiles_y, img_tiles, splits, items;
+    int kblocks;
     int stages, stage_bytes;
-    int upsample;
-    unsigned long long mg_splits, mg_tx, mg_ty;
+    int upsample;                    // CONV: store the tile through all four views (nearest x2)
+    int phased;                      // DECONV / UPCONV: phase q stores through view q only
+    ConvPhase ph[4];
+    int group_code[4];               // phases of item group g, 4 bits each, first in the low bits, ended by 0xF
+    unsigned long long mg_splits, mg_tx, mg_ty, mg_img;
     const float2* affine;            // [splits * bn / 2] x (scale, scale, bias, bias) of a channel pair, zero padded
 };
 
@@ -42,7 +50,7 @@ struct ConvBarriers {
 };
 static_assert(sizeof(ConvBarriers) <= kConvBarrierBytes, "the planner budgets the barrier block");
 
-struct ConvCoord { int img0, oy0, ox0, n0; };
+struct ConvCoord { int img0, oy0, ox0, n0, code; };
 __device__ __forceinline__ ConvCoord conv_decode(const ConvParams& p, int w, int bn) {
     ConvCoord c;
     const uint32_t t = fdiv40((uint32_t)w, p.mg_splits);
@@ -51,7 +59,9 @@ __device__ __forceinline__ ConvCoord conv_decode(const ConvParams& p, int w, int
     const int tx = (int)(t - t2 * (uint32_t)p.tiles_x);
     const uint32_t t3 = fdiv40(t2, p.mg_ty);
     const int ty = (int)(t2 - t3 * (uint32_t)p.tiles_y);
-    c.img0 = (int)t3 * p.ni; c.oy0 = ty * p.th; c.ox0 = tx * p.tw; c.n0 = split * bn;
+    const uint32_t t4 = fdiv40(t3, p.mg_img);
+    c.code = p.group_code[t4];
+    c.img0 = (int)(t3 - t4 * (uint32_t)p.img_tiles) * p.ni; c.oy0 = ty * p.th; c.ox0 = tx * p.tw; c.n0 = split * bn;
     return c;
 }
 
@@ -59,7 +69,8 @@ template <typename T, int BN, bool RELU6>
 __global__ void __launch_bounds__(CV_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
                const __grid_constant__ CUtensorMap tm_o0, const __grid_constant__ CUtensorMap tm_o1,
-               const __grid_constant__ CUtensorMap tm_o2, const __grid_constant__ CUtensorMap tm_o3, const ConvParams p) {
+               const __grid_constant__ CUtensorMap tm_o2, const __grid_constant__ CUtensorMap tm_o3,
+               const __grid_constant__ ConvParams p) {
     using MF = MixFma<T>;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -76,7 +87,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
     }
     if (warp == CV_WARP_TMA && lane == 0) {
         tma_prefetch_desc(&tm_in); tma_prefetch_desc(&tm_w); tma_prefetch_desc(&tm_o0);
-        if (p.upsample) { tma_prefetch_desc(&tm_o1); tma_prefetch_desc(&tm_o2); tma_prefetch_desc(&tm_o3); }
+        if (p.upsample || p.phased) { tma_prefetch_desc(&tm_o1); tma_prefetch_desc(&tm_o2); tma_prefetch_desc(&tm_o3); }
     }
     pdl_launch_dependents();                       // the next kernel may begin its own prologue
     pdl_wait_prior_grid();                         // everything below reads what the previous kernel wrote
@@ -88,15 +99,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
             Ring r;
             for (int w = blockIdx.x; w < p.items; w += gridDim.x) {
                 const ConvCoord c = conv_decode(p, w, BN);
-                for (int ky = 0; ky < p.ks; ++ky)
-                    for (int kx = 0; kx < p.ks; ++kx)
-                        for (int kb = 0; kb < p.kblocks; ++kb, r.next((uint32_t)p.stages)) {
-                            const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes, bar = smem_u32(&bars->full[r.s]);
-                            mbar_wait(smem_u32(&bars->empty[r.s]), r.ph ^ 1u);
-                            mbar_expect_tx(bar, (uint32_t)p.stage_bytes);
-                            tma_load_4d(st, &tm_in, bar, kb * 64, c.ox0 + kx - p.pad, c.oy0 + ky - p.pad, c.img0);
-                            tma_load_3d(st + CV_A_BYTES, &tm_w, bar, kb * 64, ky * p.ks + kx, c.n0);
-                        }
+                for (int code = c.code; code != 0xF; code >>= 4) {
+                    const ConvPhase f = p.ph[code & 0xF];
+                    for (int ky = 0; ky < f.ny; ++ky)
+                        for (int kx = 0; kx < f.nx; ++kx)
+                            for (int kb = 0; kb < p.kblocks; ++kb, r.next((uint32_t)p.stages)) {
+                                const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes, bar = smem_u32(&bars->full[r.s]);
+                                mbar_wait(smem_u32(&bars->empty[r.s]), r.ph ^ 1u);
+                                mbar_expect_tx(bar, (uint32_t)p.stage_bytes);
+                                tma_load_4d(st, &tm_in, bar, kb * 64, c.ox0 + f.dx0 + kx, c.oy0 + f.dy0 + ky, c.img0);
+                                tma_load_3d(st + CV_A_BYTES, &tm_w, bar, kb * 64, f.tap0 + ky * f.nx + kx, c.n0);
+                            }
+                }
             }
         }
     } else {
@@ -112,62 +126,66 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
         uint32_t stg_flip = 0;
         for (int w = blockIdx.x; w < p.items; w += gridDim.x) {
             const ConvCoord c = conv_decode(p, w, BN);
-            float acc[BN / 2];
+            for (int code = c.code; code != 0xF; code >>= 4) {        // the phases of this item's group, one after the other
+                const int q = code & 0xF;
+                const int ksteps = p.ph[q].ny * p.ph[q].nx * p.kblocks;
+                float acc[BN / 2];
 #pragma unroll
-            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-            uint32_t prev = 0;
-            for (int k = 0; k < p.ksteps; ++k) {
-                mbar_wait(smem_u32(&bars->full[r.s]), r.ph);
-                const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes;
-                const uint32_t a_lo = sw128_desc_lo(st + (uint32_t)wg * 8192u), b_lo = sw128_desc_lo(st + CV_A_BYTES);
-                wgmma_fence();
+                for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+                uint32_t prev = 0;
+                for (int k = 0; k < ksteps; ++k) {
+                    mbar_wait(smem_u32(&bars->full[r.s]), r.ph);
+                    const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes;
+                    const uint32_t a_lo = sw128_desc_lo(st + (uint32_t)wg * 8192u), b_lo = sw128_desc_lo(st + CV_A_BYTES);
+                    wgmma_fence();
 #pragma unroll
-                for (int k4 = 0; k4 < 4; ++k4)             // +32 B (16 channels) per K step inside the 128-byte swizzle row
-                    wgmma_bn<T, BN>(acc, sw128_desc(a_lo + 2u * k4), sw128_desc(b_lo + 2u * k4), (k > 0 || k4 > 0) ? 1u : 0u);
-                wgmma_commit();
-                wgmma_wait1();                             // the previous step's MMAs are done: release its stage
-                if (k > 0 && leader) mbar_arrive(smem_u32(&bars->empty[prev]));
-                prev = r.s;
-                r.next((uint32_t)p.stages);
-            }
-            wgmma_wait0();
-            if (leader) mbar_arrive(smem_u32(&bars->empty[prev]));
-
-            // per block of 64 output channels: registers -> BN affine + act -> 16-bit -> shared staging tile [128 px][64 ch]
-            // (16-byte chunks XOR-swizzled like a SWIZZLE_128B box) -> TMA tensor stores; image borders and the channel tail
-            // are clipped by the hardware
-#pragma unroll
-            for (int cb = 0; cb < BN / 64; ++cb) {
-                if (c.n0 + cb * 64 >= p.c_out) break;
-                uint8_t* stg = smem + stg_off + (stg_flip & 1u) * (uint32_t)kConvStg;
-                ++stg_flip;
-                const float2* aff = p.affine + c.n0 + cb * 64;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {              // 8-column group i of this block: the thread's channel pair of rows r0, r0 + 8
-                    const float4 af = __ldg(reinterpret_cast<const float4*>(aff + i * 8 + cq));     // (s0, s1, b0, b1)
-                    const f32x2 sc = f32x2_make(af.x, af.y), bi = f32x2_make(af.z, af.w);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int rr = r0 + 8 * h;
-                        const int j = cb * 8 + i;
-                        *reinterpret_cast<uint32_t*>(stg + rr * 128 + ((i ^ (rr & 7)) << 4) + cq * 2) =
-                            MF::template pack_act<RELU6>(ffma2_abc(f32x2_make(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]), sc, bi));
-                    }
+                    for (int k4 = 0; k4 < 4; ++k4)             // +32 B (16 channels) per K step inside the 128-byte swizzle row
+                        wgmma_bn<T, BN>(acc, sw128_desc(a_lo + 2u * k4), sw128_desc(b_lo + 2u * k4), (k > 0 || k4 > 0) ? 1u : 0u);
+                    wgmma_commit();
+                    wgmma_wait1();                             // the previous step's MMAs are done: release its stage
+                    if (k > 0 && leader) mbar_arrive(smem_u32(&bars->empty[prev]));
+                    prev = r.s;
+                    r.next((uint32_t)p.stages);
                 }
-                // before the OTHER staging buffer may be overwritten its previous store must have finished reading it
-                fence_proxy_async();
-                if (elected) bulk_wait_read0();
-                asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");
-                if (elected) {
-                    const uint32_t src = smem_u32(stg);
-                    const int cc = c.n0 + cb * 64;
-                    tma_store_4d(&tm_o0, src, cc, c.ox0, c.oy0, c.img0);
-                    if (p.upsample) {
-                        tma_store_4d(&tm_o1, src, cc, c.ox0, c.oy0, c.img0);
-                        tma_store_4d(&tm_o2, src, cc, c.ox0, c.oy0, c.img0);
-                        tma_store_4d(&tm_o3, src, cc, c.ox0, c.oy0, c.img0);
+                wgmma_wait0();
+                if (leader) mbar_arrive(smem_u32(&bars->empty[prev]));
+
+                // per block of 64 output channels: registers -> BN affine + act -> 16-bit -> shared staging tile [128 px][64 ch]
+                // (16-byte chunks XOR-swizzled like a SWIZZLE_128B box) -> TMA tensor stores; image borders and the channel tail
+                // are clipped by the hardware
+#pragma unroll
+                for (int cb = 0; cb < BN / 64; ++cb) {
+                    if (c.n0 + cb * 64 >= p.c_out) break;
+                    uint8_t* stg = smem + stg_off + (stg_flip & 1u) * (uint32_t)kConvStg;
+                    ++stg_flip;
+                    const float2* aff = p.affine + c.n0 + cb * 64;
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {              // 8-column group i of this block: the thread's channel pair of rows r0, r0 + 8
+                        const float4 af = __ldg(reinterpret_cast<const float4*>(aff + i * 8 + cq));     // (s0, s1, b0, b1)
+                        const f32x2 sc = f32x2_make(af.x, af.y), bi = f32x2_make(af.z, af.w);
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int rr = r0 + 8 * h;
+                            const int j = cb * 8 + i;
+                            *reinterpret_cast<uint32_t*>(stg + rr * 128 + ((i ^ (rr & 7)) << 4) + cq * 2) =
+                                MF::template pack_act<RELU6>(ffma2_abc(f32x2_make(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]), sc, bi));
+                        }
                     }
-                    bulk_commit_group();
+                    // before the OTHER staging buffer may be overwritten its previous store must have finished reading it
+                    fence_proxy_async();
+                    if (elected) bulk_wait_read0();
+                    asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");
+                    if (elected) {
+                        const uint32_t src = smem_u32(stg);
+                        const int cc = c.n0 + cb * 64;
+                        tma_store_4d(q == 0 ? &tm_o0 : q == 1 ? &tm_o1 : q == 2 ? &tm_o2 : &tm_o3, src, cc, c.ox0, c.oy0, c.img0);
+                        if (p.upsample) {
+                            tma_store_4d(&tm_o1, src, cc, c.ox0, c.oy0, c.img0);
+                            tma_store_4d(&tm_o2, src, cc, c.ox0, c.oy0, c.img0);
+                            tma_store_4d(&tm_o3, src, cc, c.ox0, c.oy0, c.img0);
+                        }
+                        bulk_commit_group();
+                    }
                 }
             }
         }
@@ -201,9 +219,10 @@ __global__ void pack_conv_affine_kernel(const float* __restrict__ scale, const f
     }
 }
 
-bool conv_tc_supported(int dtype, const StageGeom& g) {
+bool conv_tc_supported(int dtype, const StageGeom& g, int kind) {
     if (dtype != FD_F16 && dtype != FD_BF16) return false;
-    if ((g.ksize != 3 && g.ksize != 5) || g.stride != 1 || g.c_in % 8 || g.c_out % 8) return false;
+    if (g.c_in % 8 || g.c_out % 8) return false;
+    if (kind == kConvKindConv && ((g.ksize != 3 && g.ksize != 5) || g.stride != 1)) return false;
     return get_tensor_map_encoder() != nullptr;
 }
 
@@ -213,23 +232,27 @@ void conv_tc_destroy(ConvTcPlan* cp) {
     delete cp;
 }
 
-ConvPlanOut conv_tc_debug_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms) {
+ConvPlanOut conv_tc_debug_plan(int kind, int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms) {
     ConvPlanIn q{};
     q.ksize = ksize; q.h_out = h_out; q.w_out = w_out; q.n = n; q.c_in = c_in; q.c_out = c_out; q.n_sms = n_sms;
-    q.force_tile = -1;
+    q.force_tile = -1; q.kind = kind;
     return plan_conv(q);
 }
 
-// FD_CONV_TILE=<index into kConvTiles> / FD_CONV_BN=64|128|256 pin the planner's choice (tests: the result must not depend on it)
-int conv_tc_prepare(int dtype, const StageGeom& g, const void* in, const void* w, const float* scale_dev, const float* bias_dev,
-                    void* out, const TcLaunchOpts& opts, ConvTcPlan** res) {
+// FD_CONV_TILE=<index into kConvTiles> / FD_CONV_BN=64|128|256 / FD_CONV_PHASE_GROUP=1|2 (phases per item of a DECONV / UPCONV
+// stage) pin the planner's choice (tests: the result must not depend on it).  `kind` is kConvKind*; a DECONV / UPCONV stage
+// passes its input map as g.h_out / g.w_out (the conv resolution) and writes the 2x map through the four phase views.
+int conv_tc_prepare(int dtype, int kind, const StageGeom& g, const void* in, const void* w, const float* scale_dev,
+                    const float* bias_dev, void* out, const TcLaunchOpts& opts, ConvTcPlan** res) {
     PFN_encodeTiled encode = get_tensor_map_encoder();
     if (!encode) return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    const bool phased = kind != kConvKindConv;
     ConvPlanIn q{};
     q.ksize = g.ksize; q.h_out = g.h_out; q.w_out = g.w_out; q.n = g.n; q.c_in = g.c_in; q.c_out = g.c_out; q.upsample = g.upsample;
-    q.n_sms = opts.n_sms; q.force_tile = -1;
+    q.n_sms = opts.n_sms; q.force_tile = -1; q.kind = kind;
     { const char* e = getenv("FD_CONV_TILE"); if (e && *e) q.force_tile = atoi(e); }
     { const char* e = getenv("FD_CONV_BN"); if (e && *e) q.force_bn = atoi(e); }
+    { const char* e = getenv("FD_CONV_PHASE_GROUP"); if (phased && e && *e) q.force_group = atoi(e); }
     const ConvPlanOut po = plan_conv(q);
     if (!po.ok) return fail(FD_ERR_UNSUPPORTED, "dense conv stage: no tile plan fits shared memory");
     ConvTcPlan* cp = new (std::nothrow) ConvTcPlan();
@@ -239,13 +262,19 @@ int conv_tc_prepare(int dtype, const StageGeom& g, const void* in, const void* w
     memset(&p, 0, sizeof(p));
     p.n = g.n; p.h = g.h_out; p.w = g.w_out; p.c_in = g.c_in; p.c_out = g.c_out;
     p.ni = po.ni; p.th = po.th; p.tw = po.tw;
-    p.tiles_x = (g.w_out + po.tw - 1) / po.tw; p.tiles_y = (g.h_out + po.th - 1) / po.th;
+    p.tiles_x = (g.w_out + po.tw - 1) / po.tw; p.tiles_y = (g.h_out + po.th - 1) / po.th; p.img_tiles = (g.n + po.ni - 1) / po.ni;
     p.splits = po.n_splits; p.items = po.items;
-    p.ks = g.ksize; p.pad = (g.ksize - 1) / 2; p.kblocks = po.kblocks; p.ksteps = g.ksize * g.ksize * po.kblocks;
+    p.kblocks = po.kblocks;
     p.stages = po.stages; p.stage_bytes = conv_stage_bytes(po.bn);
-    p.upsample = g.upsample;
+    p.upsample = g.upsample; p.phased = phased ? 1 : 0;
+    memcpy(p.ph, po.ph, sizeof(p.ph));
+    for (int g = 0; g < 4; ++g) {
+        p.group_code[g] = 0xF;
+        for (int j = 1; j >= 0; --j)
+            if (po.group_ph[g][j] >= 0) p.group_code[g] = (p.group_code[g] << 4) | po.group_ph[g][j];
+    }
     auto magic = [](int d) { return (unsigned long long)((1ULL << 40) / (unsigned long long)d) + 1ULL; };
-    p.mg_splits = magic(p.splits); p.mg_tx = magic(p.tiles_x); p.mg_ty = magic(p.tiles_y);
+    p.mg_splits = magic(p.splits); p.mg_tx = magic(p.tiles_x); p.mg_ty = magic(p.tiles_y); p.mg_img = magic(p.img_tiles);
     const int n_pad = p.splits * po.bn;
     if (cudaMalloc(&cp->affine, (size_t)n_pad * sizeof(float2)) != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cudaMalloc failed"); }
     pack_conv_affine_kernel<<<(n_pad + 127) / 128, 128>>>(scale_dev, bias_dev, cp->affine, g.c_out, n_pad);
@@ -264,7 +293,7 @@ int conv_tc_prepare(int dtype, const StageGeom& g, const void* in, const void* w
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(conv input) failed: " + std::to_string((int)r)); }
     }
-    {   // weights [c_out][k*k][c_in] viewed as (C_in, taps, C_out); box (64, 1, bn) lands as bn K-major rows of 128 B
+    {   // weights [c_out][k*k][c_in] (phase-major taps) viewed as (C_in, taps, C_out); box (64, 1, bn) lands as bn K-major rows
         const int taps = g.ksize * g.ksize;
         cuuint64_t dims[3] = {(cuuint64_t)g.c_in, (cuuint64_t)taps, (cuuint64_t)g.c_out};
         cuuint64_t strides[2] = {(cuuint64_t)g.c_in * es, (cuuint64_t)taps * g.c_in * es};
@@ -274,13 +303,14 @@ int conv_tc_prepare(int dtype, const StageGeom& g, const void* in, const void* w
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(conv weights) failed: " + std::to_string((int)r)); }
     }
-    // output views: plain NHWC, or the four (dy, dx) phases of the 2x nearest-upsampled tensor
+    // output views: plain NHWC, or the four (dy, dx) phases of the 2x map (nearest upsample, or the phases of a DECONV / UPCONV)
     memset(cp->tm_o, 0, sizeof(cp->tm_o));
     {
-        const int up = g.upsample ? 2 : 1;
+        const bool views4 = g.upsample || phased;
+        const int up = views4 ? 2 : 1;
         const cuuint64_t P = (cuuint64_t)(g.out_pitch > 0 ? g.out_pitch : g.c_out);
         const cuuint64_t W2 = (cuuint64_t)g.w_out * up, H2 = (cuuint64_t)g.h_out * up;
-        for (int d = 0; d < (g.upsample ? 4 : 1); ++d) {
+        for (int d = 0; d < (views4 ? 4 : 1); ++d) {
             char* base = reinterpret_cast<char*>(out) + ((size_t)(d >> 1) * W2 + (d & 1)) * P * es;
             cuuint64_t dims[4] = {(cuuint64_t)g.c_out, (cuuint64_t)g.w_out, (cuuint64_t)g.h_out, (cuuint64_t)g.n};
             cuuint64_t strides[3] = {up * P * es, up * W2 * P * es, H2 * W2 * P * es};
@@ -294,8 +324,13 @@ int conv_tc_prepare(int dtype, const StageGeom& g, const void* in, const void* w
     cp->smem_bytes = (size_t)po.smem_bytes;
     cp->grid = dim3((unsigned)(p.items < opts.n_sms ? p.items : opts.n_sms), 1, 1);
     char buf[160];
-    snprintf(buf, sizeof(buf), "conv_tc_kernel<k%d,bn%d,%s>[%dx%dx%d,n%d,st%d,%s]", g.ksize, po.bn, g.upsample ? "up" : "noup",
-             po.ni, po.th, po.tw, p.splits, p.stages, g.act == FD_ACT_RELU6 ? "relu6" : "relu");
+    if (!phased)
+        snprintf(buf, sizeof(buf), "conv_tc_kernel<k%d,bn%d,%s>[%dx%dx%d,n%d,st%d,%s]", g.ksize, po.bn, g.upsample ? "up" : "noup",
+                 po.ni, po.th, po.tw, p.splits, p.stages, g.act == FD_ACT_RELU6 ? "relu6" : "relu");
+    else   // 4ph: one phase per item; 4ph2: the diagonal phase pairs
+        snprintf(buf, sizeof(buf), "conv_tc_kernel<%s%d,bn%d,%s>[%dx%dx%d,n%d,st%d,%s]", kind == kConvKindDeconv ? "deconv" : "upconv",
+                 g.ksize, po.bn, po.groups == 2 ? "4ph2" : "4ph", po.ni, po.th, po.tw, p.splits, p.stages,
+                 g.act == FD_ACT_RELU6 ? "relu6" : "relu");
     cp->name = buf;
     *res = cp;
     return FD_OK;

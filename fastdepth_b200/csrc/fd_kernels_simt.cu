@@ -6,6 +6,8 @@
 //                   upsample + skip add in the epilogue               (reference imagenet/mobilenet.py:35-37; models.py:70-75,723-729)
 //  * conv_kernel  : dense kxk stride-1 conv+BN+act (+ nearest x2 upsample) of the dense NNConv decoder
 //                                                                      (reference models.py:52-59, 245-270)
+//  * convt_kernel : transposed conv / unpool + 5x5 conv, +BN+act, of the DeConv and UpConv decoders, one output phase per
+//                   grid z                                            (reference models.py:18-34, 77-107, 145-201)
 //  * head_kernel  : pointwise(C,1)+BN+ReLU -> [N,1,H,W] (optionally below the last upsample)
 //                                                                      (reference models.py:698,731)
 //
@@ -14,6 +16,7 @@
 // block kernel in fd_block_tc.cu).  All accumulate in fp32 and apply BN as a folded fp32
 // per-channel affine, then round once to the storage dtype.
 #include "fd_common.cuh"
+#include "fd_conv_plan.h"
 
 namespace fd {
 
@@ -324,6 +327,88 @@ conv_kernel(const T* __restrict__ in, const T* __restrict__ wgt, T* __restrict__
 }
 
 // ----------------------------------------------------------------------------------------
+// transposed conv (DECONV) / unpool + conv (UPCONV) + BN + act, path 0: blockIdx.z is the output phase q = 2 ry + rx; the GEMM
+// above over the n*h*w input-resolution pixels (Y, X) with K = that phase's taps * c_in, the A row of (Y, X) gathered at
+// (Y + dy, X + dx) (only the taps the phase really has), the result stored at output pixel (2 Y + ry, 2 X + rx).  Weights
+// [c_out][k*k][c_in] with phase-major taps (fd_conv_plan.h).
+// ----------------------------------------------------------------------------------------
+struct ConvPhases { ConvPhase ph[4]; };
+
+template <typename T>
+__global__ void __launch_bounds__(PW_THREADS)
+convt_kernel(const T* __restrict__ in, const T* __restrict__ wgt, T* __restrict__ out,
+             const float* __restrict__ scale, const float* __restrict__ bias,
+             int n, int h, int w, int c_in, int c_out, int in_pitch, int out_pitch, int taps, const ConvPhases phs, int act) {
+    __shared__ float As[PW_BK][PW_BM + 4];
+    __shared__ float Ws[PW_BK][PW_BN + 4];
+    const int q = blockIdx.z;
+    const ConvPhase f = phs.ph[q];
+    const int tid = threadIdx.x;
+    const long long m_total = (long long)n * h * w;
+    const long long m0 = (long long)blockIdx.x * PW_BM;
+    const int n0 = blockIdx.y * PW_BN;
+    const int lr = tid >> 2;
+    const int lk = (tid & 3) * 4;
+    const int ty = tid >> 4, tx = tid & 15;
+    const int k_total = f.ny * f.nx * c_in;
+    const long long lm = m0 + lr;
+    const int lx = (int)(lm % w);
+    const int ly = (int)((lm / w) % h);
+    const long long limg = lm / ((long long)w * h);
+
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+
+    for (int k0 = 0; k0 < k_total; k0 += PW_BK) {
+        float va[4] = {0.f, 0.f, 0.f, 0.f}, vw[4] = {0.f, 0.f, 0.f, 0.f};
+        const int kk = k0 + lk;
+        if (kk < k_total) {
+            const int tap = kk / c_in, ci = kk - tap * c_in;
+            const int iy = ly + f.dy0 + tap / f.nx, ix = lx + f.dx0 + tap % f.nx;
+            if (lm < m_total && iy >= 0 && iy < h && ix >= 0 && ix < w)
+                load4f<T>(in + (((size_t)limg * h + iy) * w + ix) * in_pitch + ci, va);
+            if (n0 + lr < c_out) load4f<T>(wgt + ((size_t)(n0 + lr) * taps + f.tap0 + tap) * c_in + ci, vw);
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { As[lk + j][lr] = va[j]; Ws[lk + j][lr] = vw[j]; }
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < PW_BK; ++k) {
+            float ra[4], rw[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) { ra[i] = As[k][ty * 4 + i]; rw[i] = Ws[k][tx * 4 + i]; }
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(ra[i], rw[j], acc[i][j]);
+        }
+        __syncthreads();
+    }
+
+    const int co = n0 + tx * 4;
+    if (co >= c_out) return;
+    float sc[4], bi[4];
+    load4f<float>(scale + co, sc);
+    load4f<float>(bias + co, bi);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const long long m = m0 + ty * 4 + i;
+        if (m >= m_total) continue;
+        float y[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) y[j] = apply_act(fmaf(acc[i][j], sc[j], bi[j]), act);
+        const int px = (int)(m % w);
+        const long long t = m / w;
+        const int py = (int)(t % h);
+        const long long img = t / h;
+        store4f<T>(out + (((size_t)img * 2 * h + 2 * py + (q >> 1)) * (2 * w) + 2 * px + (q & 1)) * out_pitch + co, y);
+    }
+}
+
+// ----------------------------------------------------------------------------------------
 // head: C -> 1 pointwise + BN + ReLU, written as [N,1,H,W]; with up=1 every low-res result is
 // replicated to its 2x2 block (decode_conv6 commutes with the last nearest upsample)
 // ----------------------------------------------------------------------------------------
@@ -413,6 +498,20 @@ static int launch_conv_t(const void* in, const void* w, void* out, const float* 
 }
 
 template <typename T>
+static int launch_convt_t(int kind, const void* in, const void* w, void* out, const float* scale, const float* bias,
+                          const StageGeom& g, cudaStream_t st) {
+    ConvPhases phs;
+    conv_phases(kind, g.ksize, phs.ph);
+    const long long m_total = (long long)g.n * g.h_out * g.w_out;
+    dim3 grid((unsigned)((m_total + PW_BM - 1) / PW_BM), (unsigned)((g.c_out + PW_BN - 1) / PW_BN), 4);
+    convt_kernel<T><<<grid, PW_THREADS, 0, st>>>((const T*)in, (const T*)w, (T*)out, scale, bias, g.n, g.h_out, g.w_out, g.c_in,
+                                                 g.c_out, g.in_pitch > 0 ? g.in_pitch : g.c_in,
+                                                 g.out_pitch > 0 ? g.out_pitch : g.c_out, g.ksize * g.ksize, phs, g.act);
+    FD_CUDA_OK(cudaGetLastError());
+    return FD_OK;
+}
+
+template <typename T>
 static int launch_head_t(const void* in, void* out, const float* w, float scale, float bias, long long m_total, int c,
                          int in_pitch, int h, int wd, int up, int act, cudaStream_t st) {
     const int threads = 256;
@@ -439,6 +538,10 @@ int launch_pw(int dtype, const BlockArgs& a, cudaStream_t st) { FD_DISPATCH(dtyp
 int launch_conv(int dtype, const void* in, const void* w, void* out, const float* scale, const float* bias, const StageGeom& g,
                 cudaStream_t st) {
     FD_DISPATCH(dtype, launch_conv_t<T>(in, w, out, scale, bias, g, st));
+}
+int launch_convt(int dtype, int kind, const void* in, const void* w, void* out, const float* scale, const float* bias,
+                 const StageGeom& g, cudaStream_t st) {
+    FD_DISPATCH(dtype, launch_convt_t<T>(kind, in, w, out, scale, bias, g, st));
 }
 int launch_head(int dtype, const void* in, void* out, const float* w, float scale, float bias, long long m_total, int c,
                 int in_pitch, int h, int wd, int up, int act, cudaStream_t st) {

@@ -68,6 +68,11 @@ def _blocks_of(module):
         return enc, dec, module.decode_conv6, ('concat' if concat else True), names
     if hasattr(module, 'mobilenet') and hasattr(module, 'decoder'):
         enc = [module.mobilenet[i] for i in range(14)]
+        for child in ('convt', 'upconv'):          # DeConv / UpConv decoders (reference models.py:145-201)
+            if hasattr(module.decoder, child + '1'):
+                dec = [getattr(module.decoder, '%s%d' % (child, j)) for j in range(1, 6)]
+                names = ['mobilenet.%d' % i for i in range(14)] + ['decoder.%s%d' % (child, j) for j in range(1, 6)]
+                return enc, dec, module.decoder.convf, False, names + ['decoder.convf']
         dec = [getattr(module.decoder, 'conv%d' % j) for j in range(1, 6)]
         names = ['mobilenet.%d' % i for i in range(14)] + ['decoder.conv%d' % j for j in range(1, 7)]
         return enc, dec, module.decoder.conv6, False, names
@@ -81,18 +86,38 @@ def _is_dense_block(b):
             _sq(b[0].kernel_size) in (3, 5) and _sq(b[0].stride) == 1 and isinstance(b[1], nn.BatchNorm2d))
 
 
+def _convt_kind(b):
+    """FD_STAGE_DECONV for convt(C, C', k) (ConvTranspose2d(k in 3/5/7/9, stride 2, padding (k-1)/2, output_padding 1),
+    BN, ReLU; reference models.py:77-87), FD_STAGE_UPCONV for upconv(C, C') (Unpool(2), Conv2d(5, 1, 2), BN, ReLU;
+    l.101-107), else None."""
+    if not isinstance(b, nn.Sequential):
+        return None
+    if len(b) == 3 and isinstance(b[0], nn.ConvTranspose2d) and isinstance(b[1], nn.BatchNorm2d):
+        c, k = b[0], _sq(b[0].kernel_size)
+        ok = (k in (3, 5, 7, 9) and c.groups == 1 and _sq(c.stride) == 2 and _sq(c.padding) == (k - 1) // 2 and
+              _sq(c.output_padding) == 1 and _sq(c.dilation) == 1 and c.bias is None)
+        return _lib.FD_STAGE_DECONV if ok else None
+    if len(b) == 4 and type(b[0]).__name__ == 'Unpool' and isinstance(b[1], nn.Conv2d) and isinstance(b[2], nn.BatchNorm2d):
+        c = b[1]
+        ok = (getattr(b[0], 'stride', None) == 2 and _sq(c.kernel_size) == 5 and c.groups == 1 and _sq(c.stride) == 1 and
+              _sq(c.padding) == 2 and _sq(c.dilation) == 1 and c.bias is None)
+        return _lib.FD_STAGE_UPCONV if ok else None
+    return None
+
+
 def dense_decoder(module):
-    """True if the module's decoder is the dense NNConv decoder (``MobileNet('nnconv5')`` / ``('nnconv3')``)."""
+    """True if the module's decoder is dense: the NNConv decoder (``MobileNet('nnconv5')`` / ``('nnconv3')``) or the
+    DeConv / UpConv decoder (``MobileNet('deconv<k>')`` / ``('upconv')``)."""
     try:
         _, dec, _, _, _ = _blocks_of(module)
-        return all(_is_dense_block(b) for b in dec)
+        return all(_is_dense_block(b) for b in dec) or all(_convt_kind(b) is not None for b in dec)
     except Exception:
         return False
 
 
 def supports(module):
-    """True if ``describe`` can express the module: depthwise-separable decoder blocks of two Sequentials, or dense
-    k x k conv blocks (k in {3, 5}) of the NNConv decoder."""
+    """True if ``describe`` can express the module: depthwise-separable decoder blocks of two Sequentials, dense
+    k x k conv blocks (k in {3, 5}) of the NNConv decoder, or the transposed-conv / unpool blocks of DeConv / UpConv."""
     try:
         enc, dec, head, _, _ = _blocks_of(module)
         return all(isinstance(b, nn.Sequential) and len(b) == 2 and isinstance(b[0], nn.Sequential) and
@@ -107,7 +132,8 @@ def describe(module):
 
     Mirrors the dispatch of reference models.py:706-732 (SkipAdd: skips saved after encoder blocks 1/3/5 and added
     after decoder stages 4/3/2) and models.py:253-270, 457-460 (MobileNet + NNConv: no skips; a dense decoder block
-    becomes one CONV stage with the weight tuple ``(None, None, None, w.reshape(c_out, -1), scale, bias)``)."""
+    becomes one CONV stage with the weight tuple ``(None, None, None, w.reshape(c_out, -1), scale, bias)``; a DeConv /
+    UpConv block becomes one DECONV / UPCONV stage with the module's own weight, flattened behind its first axis)."""
     enc, dec, hd, with_skips, names = _blocks_of(module)
     descs, weights = [], []
     conv0 = enc[0]
@@ -131,6 +157,17 @@ def describe(module):
         stage_of_encoder[i] = len(descs) - 1
     for j in range(1, 6):
         blk = dec[j - 1]
+        kind = _convt_kind(blk)
+        if kind is not None:
+            # convt(): ConvTranspose2d weights [c_in][c_out][k][k]; upconv(): Unpool, then Conv2d weights [c_out][c_in][5][5]
+            c, bn, a = (blk[0], blk[1], blk[2]) if kind == _lib.FD_STAGE_DECONV else (blk[1], blk[2], blk[3])
+            c_in, c_out = (c.weight.shape[0], c.weight.shape[1]) if kind == _lib.FD_STAGE_DECONV else \
+                (c.weight.shape[1], c.weight.shape[0])
+            descs.append(dict(kind=kind, c_in=c_in, c_out=c_out, ksize=_sq(c.kernel_size), stride=2, act=_act_of(a),
+                              upsample=0, skip_src=-1))
+            s, b = fold_bn(bn)
+            weights.append((None, None, None, _w(c).reshape(c.weight.shape[0], -1), s, b))
+            continue
         if _is_dense_block(blk):
             # dense kxk conv + BN + ReLU, then the nearest x2 upsample (reference models.py:52-59, 261-270)
             c, bn, a = blk[0], blk[1], blk[2]

@@ -216,3 +216,71 @@ def synthetic_nnconv_state_dict(kernel_size=5, seed=1, calib_hw=(96, 128)):
     sd['decoder.conv6.0.weight'] = torch.from_numpy(np.abs(rng.uniform(-b, b, (1, c, 1, 1)))).float().contiguous()
     calibrate(F.conv2d(x, sd['decoder.conv6.0.weight'].to(f64)), 'decoder.conv6.1', last=True)
     return sd
+
+
+def synthetic_convt_state_dict(decoder, seed=1, calib_hw=(96, 128)):
+    """state_dict with the ``models.MobileNet(decoder)`` key schema for ``decoder`` in ``deconv3/5/7/9`` and ``upconv``
+    (reference models.py:77-107, 145-201): the encoder of ``synthetic_state_dict(STOCK_WIDTHS, seed)`` (renamed with
+    ``to_mobilenet_keys``), then five ``convt(C, C/2, k)`` (keys ``decoder.convt<j>.{0,1}.*``) or ``upconv(C, C/2)``
+    blocks (``decoder.upconv<j>.{1,2}.*``) and ``convf = pointwise(32, 1)``, drawn from a separate seeded stream.
+
+    The recipe of ``synthetic_nnconv_state_dict``: decoder weights U(-b, b) with b = 1/sqrt(k*k*C), BN gamma / beta drawn
+    as there, running statistics CALIBRATED in fp64 on the same probe batch, a positive head with gamma = 1, beta = 3."""
+    import torch.nn.functional as F
+    if decoder == 'upconv':
+        k, child, conv_i, bn_i = 5, 'upconv', 1, 2
+    elif decoder in ('deconv3', 'deconv5', 'deconv7', 'deconv9'):
+        k, child, conv_i, bn_i = int(decoder[6]), 'convt', 0, 1
+    else:
+        raise ValueError('no synthetic recipe for decoder %r' % decoder)
+    base = to_mobilenet_keys(synthetic_state_dict(STOCK_WIDTHS, seed=seed, calib_hw=calib_hw))
+    sd = {key: v for key, v in base.items() if key.startswith('mobilenet.')}
+    f64 = torch.float64
+
+    def bn(t, prefix, hi):
+        g, b = sd[prefix + '.weight'].to(f64), sd[prefix + '.bias'].to(f64)
+        m, v = sd[prefix + '.running_mean'].to(f64), sd[prefix + '.running_var'].to(f64)
+        inv = g / torch.sqrt(v + 1e-5)
+        y = t * inv.view(1, -1, 1, 1) + (b - m * inv).view(1, -1, 1, 1)
+        return y.clamp(0.0, hi) if hi is not None else y.clamp_min(0.0)
+
+    strides = (2, 1, 2, 1, 2, 1, 2, 1, 1, 1, 1, 1, 2, 1)
+    x = torch.from_numpy(np.random.Generator(np.random.PCG64(seed + 7919)).random((2, 3) + tuple(calib_hw)))
+    x = bn(F.conv2d(x, sd['mobilenet.0.0.weight'].to(f64), None, 2, 1), 'mobilenet.0.1', 6.0)
+    for i in range(1, 14):
+        ci = sd['mobilenet.%d.0.weight' % i].shape[0]
+        x = bn(F.conv2d(x, sd['mobilenet.%d.0.weight' % i].to(f64), None, strides[i], 1, 1, ci), 'mobilenet.%d.1' % i, 6.0)
+        x = bn(F.conv2d(x, sd['mobilenet.%d.3.weight' % i].to(f64)), 'mobilenet.%d.4' % i, 6.0)
+    rng = np.random.Generator(np.random.PCG64(seed + 104729))
+    c = STOCK_ENCODER[13]
+
+    def calibrate(t, prefix, last=False):
+        ch = t.shape[1]
+        if last:
+            gamma, beta = np.ones(ch), np.full(ch, 3.0)
+        else:
+            gamma, beta = rng.uniform(GAMMA_RANGE[0], GAMMA_RANGE[1], ch), rng.normal(BETA[0], BETA[1], ch)
+        sd[prefix + '.weight'] = torch.from_numpy(gamma).float()
+        sd[prefix + '.bias'] = torch.from_numpy(beta).float()
+        sd[prefix + '.running_mean'] = t.mean(dim=(0, 2, 3)).float()
+        sd[prefix + '.running_var'] = t.var(dim=(0, 2, 3), unbiased=False).float()
+        sd[prefix + '.num_batches_tracked'] = torch.zeros((), dtype=torch.int64)
+        return bn(t, prefix, None)
+
+    for j, co in enumerate(STOCK_DECODER, start=1):
+        b = 1.0 / np.sqrt(k * k * c)
+        key = 'decoder.%s%d.%d.weight' % (child, j, conv_i)
+        if child == 'convt':
+            sd[key] = torch.from_numpy(rng.uniform(-b, b, (c, co, k, k))).float().contiguous()
+            y = F.conv_transpose2d(x, sd[key].to(f64), None, 2, (k - 1) // 2, 1)
+        else:
+            sd[key] = torch.from_numpy(rng.uniform(-b, b, (co, c, k, k))).float().contiguous()
+            u = x.new_zeros(x.shape[0], c, x.shape[2], 2, x.shape[3], 2)
+            u[:, :, :, 0, :, 0] = x
+            y = F.conv2d(u.view(x.shape[0], c, 2 * x.shape[2], 2 * x.shape[3]), sd[key].to(f64), None, 1, 2)
+        x = calibrate(y, 'decoder.%s%d.%d' % (child, j, bn_i))
+        c = co
+    b = 1.0 / np.sqrt(c)
+    sd['decoder.convf.0.weight'] = torch.from_numpy(np.abs(rng.uniform(-b, b, (1, c, 1, 1)))).float().contiguous()
+    calibrate(F.conv2d(x, sd['decoder.convf.0.weight'].to(f64)), 'decoder.convf.1', last=True)
+    return sd

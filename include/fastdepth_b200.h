@@ -57,9 +57,17 @@ typedef enum {
                              depthwise+pointwise, reference models.py:61-75, 683-697)        */
     FD_STAGE_HEAD = 2,   /* pointwise C->1 + BN + act, NHWC in -> [N,1,H,W] out
                             (decode_conv6, reference models.py:698, 731)                     */
-    FD_STAGE_CONV = 3    /* dense kxk (k in {3,5}) stride-1 conv, padding (k-1)/2, + BN + act, then the
+    FD_STAGE_CONV = 3,   /* dense kxk (k in {3,5}) stride-1 conv, padding (k-1)/2, + BN + act, then the
                             optional nearest x2 upsample; NHWC in -> NHWC out.  No skip, no stride 2
                             (conv() blocks of the dense NNConv decoder, reference models.py:52-59, 245-270) */
+    FD_STAGE_DECONV = 4, /* ConvTranspose2d(c_in, c_out, k, stride 2, padding (k-1)/2, output_padding 1), k in
+                            {3,5,7,9}, + BN + act; NHWC [N,h,w,c_in] in -> NHWC [N,2h,2w,c_out] out.  stride must
+                            be 2, upsample 0, skip_src -1 (convt() blocks of the DeConv decoder, reference
+                            models.py:77-87, 145-180) */
+    FD_STAGE_UPCONV = 5  /* 2x2 zero-insertion unpool, then a 5x5 stride-1 conv with padding 2, + BN + act;
+                            NHWC [N,h,w,c_in] in -> NHWC [N,2h,2w,c_out] out.  ksize 5, stride 2, upsample 0,
+                            skip_src -1 (upconv() blocks of the UpConv decoder, reference models.py:18-34,
+                            101-107, 183-201) */
 } fd_stage_kind;
 
 typedef enum { FD_ACT_RELU = 0, FD_ACT_RELU6 = 1 } fd_act;
@@ -79,7 +87,7 @@ typedef struct {
                             models.py:806-811) -- the next stage then has c_in = c_out + c_skip  */
 } fd_stage_desc;
 
-/* Build a plan for a stage list (always: 1 STEM, k stages each DWPW or CONV, 1 HEAD) at a fixed problem size.
+/* Build a plan for a stage list (always: 1 STEM, k stages each DWPW, CONV, DECONV or UPCONV, 1 HEAD) at a fixed problem size.
  * Allocates NHWC activation buffers and packed-weight storage on `device`.
  * H and W must be multiples of 32 (reference forward's skip shapes only line up then),
  * every c_in/c_out except the stem's c_in and the head's c_out a multiple of 8. */
@@ -94,6 +102,9 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages,
  *   DWPW : dw_w = [c_in][k][k], dw_scale/dw_bias = [c_in] ; pw_w = [c_out][c_in], pw_scale/pw_bias = [c_out]
  *   CONV : dw_* = NULL ; pw_w = [c_out][c_in][k][k]  ; pw_scale/pw_bias = [c_out]  (PyTorch's layout; the
  *          plan keeps it as [c_out][k*k][c_in] in the plan dtype, the K-major operand both conv kernels read)
+ *   DECONV: dw_* = NULL ; pw_w = [c_in][c_out][k][k] (PyTorch's ConvTranspose2d layout) ; pw_scale/pw_bias = [c_out]
+ *   UPCONV: dw_* = NULL ; pw_w = [c_out][c_in][5][5] ; pw_scale/pw_bias = [c_out]
+ *          (both are kept as [c_out][k*k][c_in], the taps grouped by output phase, i.e. by the parity of the output pixel)
  *   HEAD : dw_* = NULL ; pw_w = [1][c_in]            ; pw_scale/pw_bias = [1]              */
 int fd_plan_set_stage_weights(fd_plan* plan, int stage,
                               const float* dw_w, const float* dw_scale, const float* dw_bias,
@@ -148,7 +159,7 @@ int fd_pipeline_wait(fd_plan* plan, unsigned long long ticket);
 /* Introspection for stage-parity tests: the NHWC buffer stage `stage` wrote in the last
  * fd_forward (valid until the next one).  c_stride = elements between pixels.
  * which = 0: the stage output (after upsample/skip-add); 1: the depthwise intermediate
- * (only materialised on path 0; a CONV stage has none and fails with FD_ERR_INVALID). */
+ * (only materialised on path 0; a CONV, DECONV or UPCONV stage has none and fails with FD_ERR_INVALID). */
 int fd_stage_buffer(fd_plan* plan, int stage, int which, void** dev_ptr,
                     int* n, int* h, int* w, int* c, int* c_stride);
 
@@ -189,6 +200,14 @@ int fd_debug_block_plan(int ksize, int stride, int h_out, int w_out, int n, int 
  * channels per item), stages (operand ring depth), m_tiles, n_splits, items, waves, kblocks (64-channel blocks per
  * tap), smem_bytes, useful_rows_permille, cost (modelled time, arbitrary units), 0, 0}.  cap must be at least 16. */
 int fd_debug_conv_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms, int* out, int cap);
+
+/* Debug (host only, needs no GPU): the same plan for a DECONV or UPCONV stage (`kind`) on an h_in x w_in input map: four
+ * stride-1 phase convs at the input resolution, items = m_tiles * n_splits * phase groups.  out[0..15] as in
+ * fd_debug_conv_plan except out[14] = the number of phase groups (4: one phase per item, 2: the diagonal pairs {00, 11} and
+ * {01, 10}); out[16 + 5 q .. 20 + 5 q] = {tap0, ny, nx, dy0, dx0} of phase q = 2 ry + rx (its taps tap0 .. tap0 + ny nx - 1
+ * of the repacked weights, input offsets dy0 .. dy0 + ny - 1 by dx0 .. dx0 + nx - 1); out[36 + 2 g .. 37 + 2 g] = the phases
+ * of group g (-1 = none), in execution order.  cap must be at least 44. */
+int fd_debug_convt_plan(int kind, int ksize, int h_in, int w_in, int n, int c_in, int c_out, int n_sms, int* out, int cap);
 
 /* Per-image depth metrics on device (reference metrics.py:31-55 applied per image, as
  * main.py:40-41,80-82 does at batch size 1).  pred: [n, hw] of `dtype`; target: [n, hw] fp32.

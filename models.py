@@ -25,7 +25,11 @@ What is here and what is not (SURVEY.md section 2 / section 8):
   conv on the implicit-GEMM wgmma kernel (fd_conv_tc.cu).  The dense decoder in fp32
   stays on stock PyTorch: the project's fp32 path is SIMT, while cuDNN may run fp32
   convolutions on TF32 tensor cores (tools/bench_nnconv5.py measures both).
-* every other decoder/encoder family of the reference (DeConv, UpConv, UpProj,
+* ``MobileNet`` + ``DeConv`` / ``UpConv``  -- the decoder ablation of the paper
+  ("MobileNet-DeConv{3,5,7,9}", "MobileNet-UpConv"): plain PyTorch on the CPU; an fp16 / bf16
+  CUDA tensor runs every transposed conv (or unpool + 5x5 conv) as four stride-1 phase convs
+  on the same wgmma kernel (DESIGN.md section 3.6b); fp32 stays on stock PyTorch.
+* every other decoder/encoder family of the reference (DeConv with depthwise convs, UpProj,
   BLConv, ShuffleConv, ResNet*) is out of scope of this tier; ``choose_decoder``
   names them in its error.
 * ``MobileNetSkipConcat``  -- SURVEY.md section 8f row 1: the concat-skip variant
@@ -83,6 +87,47 @@ def _cbr(c_in, c_out, k, groups=1):
         nn.ReLU(inplace=True))
 
 
+class Unpool(nn.Module):
+    """x2 unpooling with zero padding (reference models.py:18-34): every input pixel lands at the top-left corner of
+    its 2x2 output block, the other three are zero.  ``mask`` ([1, 0; 0, 0]) is a plain attribute, not a buffer, as in the
+    reference, so that whole-module pickles and state_dicts keep their keys."""
+
+    def __init__(self, stride=2):
+        super().__init__()
+        self.stride = stride
+        self.mask = torch.zeros(1, 1, stride, stride)
+        self.mask[:, :, 0, 0] = 1
+
+    def forward(self, x):
+        assert x.dim() == 4
+        n, c, h, w = x.shape
+        s = self.stride
+        out = x.new_zeros(n, c, h, s, w, s)
+        out[:, :, :, 0, :, 0] = x
+        return out.view(n, c, h * s, w * s)
+
+
+def convt(in_channels, out_channels, kernel_size):
+    """ConvTranspose2d(k, stride 2, padding (k-1)/2, output_padding k % 2) + BN + ReLU: exactly x2 (reference
+    models.py:77-87)."""
+    pad, out_pad = (kernel_size - 1) // 2, kernel_size % 2
+    if kernel_size + out_pad - 2 * pad != 2:
+        raise AssertionError("deconv parameters incorrect")
+    return nn.Sequential(
+        nn.ConvTranspose2d(in_channels, out_channels, kernel_size, 2, pad, out_pad, bias=False),
+        nn.BatchNorm2d(out_channels),
+        nn.ReLU(inplace=True))
+
+
+def upconv(in_channels, out_channels):
+    """Unpool(2) -> 5x5 conv -> BN -> ReLU (reference models.py:101-107)."""
+    return nn.Sequential(
+        Unpool(2),
+        nn.Conv2d(in_channels, out_channels, kernel_size=5, stride=1, padding=2, bias=False),
+        nn.BatchNorm2d(out_channels),
+        nn.ReLU())
+
+
 def conv(in_channels, out_channels, kernel_size):
     """Dense kxk conv + BN + ReLU (reference models.py:52-59)."""
     return _cbr(in_channels, out_channels, kernel_size)
@@ -123,21 +168,66 @@ class NNConv(nn.Module):
         return self.conv6(x)
 
 
-_OUT_OF_SCOPE_DECODERS = ('deconv', 'upproj', 'upconv', 'shuffle', 'blconv')
+_DECODER_CHANNELS = (1024, 512, 256, 128, 64, 32)
+
+
+class DeConv(nn.Module):
+    """5 x convt(C, C/2, k) + pointwise(32, 1) (reference models.py:145-180), children ``convt1..5`` and ``convf``.  The
+    depthwise variant (``deconv<k>dw``) is not built here."""
+
+    def __init__(self, kernel_size, dw):
+        super().__init__()
+        if dw:
+            raise NotImplementedError("decoder 'deconv%ddw' is out of scope of the H100 hot-path build; see DESIGN.md"
+                                      % kernel_size)
+        ch = _DECODER_CHANNELS
+        for i in range(5):
+            setattr(self, 'convt%d' % (i + 1), convt(ch[i], ch[i + 1], kernel_size))
+        self.convf = pointwise(ch[5], 1)
+
+    def forward(self, x):
+        for i in range(1, 6):
+            x = getattr(self, 'convt%d' % i)(x)
+        return self.convf(x)
+
+
+class UpConv(nn.Module):
+    """5 x upconv(C, C/2) + pointwise(32, 1) (reference models.py:183-201), children ``upconv1..5`` and ``convf``."""
+
+    def __init__(self):
+        super().__init__()
+        ch = _DECODER_CHANNELS
+        for i in range(5):
+            setattr(self, 'upconv%d' % (i + 1), upconv(ch[i], ch[i + 1]))
+        self.convf = pointwise(ch[5], 1)
+
+    def forward(self, x):
+        for i in range(1, 6):
+            x = getattr(self, 'upconv%d' % i)(x)
+        return self.convf(x)
+
+
+_OUT_OF_SCOPE_DECODERS = ('upproj', 'shuffle', 'blconv')
 
 
 def choose_decoder(decoder):
     """String -> decoder factory (reference models.py:335-360).
 
-    ``nnconv<k>`` / ``nnconv<k>dw`` are supported; the ablation decoders of the paper are
-    outside this build's scope (SURVEY.md section 2) and raise NotImplementedError."""
+    ``nnconv<k>`` / ``nnconv<k>dw``, ``deconv<k>`` (k in 3, 5, 7, 9) and ``upconv`` are supported; ``deconv<k>dw`` and the
+    other ablation decoders of the paper are outside this build's scope (SURVEY.md section 2) and raise
+    NotImplementedError."""
     use_dw = 'dw' in decoder
     if decoder[:6] == 'nnconv':
         assert len(decoder) == 7 or (len(decoder) == 9 and use_dw)
         model = NNConv(int(decoder[6]), use_dw)
+    elif decoder[:6] == 'deconv':
+        assert len(decoder) == 7 or (len(decoder) == 9 and use_dw)
+        model = DeConv(int(decoder[6]), use_dw)
+    elif decoder == 'upconv':
+        model = UpConv()
     elif any(decoder.startswith(p) for p in _OUT_OF_SCOPE_DECODERS):
         raise NotImplementedError(
-            "decoder '%s' is out of scope of the H100 hot-path build (only nnconv*); see DESIGN.md" % decoder)
+            "decoder '%s' is out of scope of the H100 hot-path build (nnconv*, deconv3/5/7/9, upconv); see DESIGN.md" % decoder)
     else:
         assert False, "invalid option for decoder: {}".format(decoder)
     model.apply(weights_init)
@@ -178,7 +268,8 @@ class MobileNet(nn.Module):
         A CUDA tensor through the depthwise NNConv decoder ("MobileNet-NNConv5(dw)", reference README.md:37) takes the same
         fused sm_90a path as MobileNetSkipAdd, just without skips.  A CUDA fp16 / bf16 tensor through the dense decoder
         ("MobileNet-NNConv5", README.md:36) takes the engine too, with the decoder convs on conv_tc_kernel; the dense
-        decoder in fp32 stays on stock PyTorch (cuDNN may use TF32 tensor cores there, the project's fp32 path is SIMT)."""
+        decoder in fp32 stays on stock PyTorch (cuDNN may use TF32 tensor cores there, the project's fp32 path is SIMT).
+        The DeConv and UpConv decoders route the same way as the dense NNConv decoder."""
         fused_ok = (x.is_cuda and not self.training and x.dim() == 4 and x.shape[1] == 3 and
                     x.shape[2] % 32 == 0 and x.shape[3] % 32 == 0)     # what the fused plan covers; anything else: stock PyTorch
         if fused_ok:
