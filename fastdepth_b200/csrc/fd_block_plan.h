@@ -12,6 +12,18 @@ constexpr int kPlanMaxACluster = 6;          // cluster mode: the A ring is fill
 // An item's accumulator lives in the registers of the two consumer warpgroups (64 pixel rows each): n_cta / 2 fp32 registers per
 // thread, so 128 output channels per item is the most the register file leaves room for next to the other roles.
 constexpr int kPlanMaxNcta = 128;
+// Bytes of the taps in a K-block's depthwise parameter block {taps, [64] fp32 scale, [64] fp32 bias}.
+//   3x3: [9][64] taps in the storage dtype.
+//   5x5: [5 kernel rows][32 lanes][6 fp32 pairs] -- per lane (channel pair) and kernel row the 5 tap pairs (kx = 0..4) and one
+//        zero pair.  The values are rounded to the storage dtype, so the products stay exact.  The depthwise loop reads a lane's
+//        kernel row with three 16-byte loads where it is used, since 25 taps held in registers do not fit beside the
+//        accumulators under the kernel's register cap; the 48-byte lane stride keeps every quarter-warp's 16-byte loads on
+//        distinct banks.
+// (The kernel reads this too, hence the device qualifier under CUDA.)
+#ifdef __CUDACC__
+__host__ __device__
+#endif
+constexpr int dw_taps_bytes(int ksize) { return ksize == 5 ? 5 * 32 * 48 : ksize * ksize * 64 * 2; }
 #ifndef FD_PLAN_SMALL_SMEM
 // everything that needs 1 KB alignment sits in front of the 128-byte-granular input stages (see the kernel's carve-up): ONE alignment
 // slack, and the budget is the whole 227 KB an H100 block may opt into, minus a small margin
@@ -114,7 +126,7 @@ inline BlockPlanOut plan_block(const BlockPlanIn& q) {
     p.kblocks = (q.c_in + kPlanKblk - 1) / kPlanKblk;
     p.cin_pad = p.kblocks * kPlanKblk;
     p.in_stage_bytes = NI * IH * IW * 128;
-    p.dwp_bytes = q.ksize * q.ksize * 128 + 512;
+    p.dwp_bytes = dw_taps_bytes(q.ksize) + 512;
     p.in_stage_stride = (p.in_stage_bytes + p.dwp_bytes + 127) / 128 * 128;
     // Split the output channels into items (each item recomputes the depthwise half for its 128 pixels and reloads the
     // input tile, so splitting is not free).  Candidates: n_cta <= 128 (the register accumulators), multiples of 64 when there

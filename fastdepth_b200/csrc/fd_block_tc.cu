@@ -80,7 +80,7 @@ struct TcParams {
     int epi_tma;          // 1: staging tiles leave through TMA tensor stores (4 strided views for nearest-x2 upsampling)
     int epi_red;          // 1: ... as element-wise ADD into the skip tensor, which then IS the block's output (in place)
     unsigned long long mg_splits, mg_tx, mg_ty;   // 2^40 / d reciprocals for the item -> tile decode
-    const void* dwp;      // [kblocks] x { [k*k][64] 16-bit taps, [64] fp32 scale, [64] fp32 bias }
+    const void* dwp;      // [kblocks] x { taps (see dw_taps_bytes), [64] fp32 scale, [64] fp32 bias }
     const float2* pw_affine;  // [cpad_all / 2] x (scale, scale, bias, bias) of a channel pair
     const float* head_w;  // [cpad_all]
     int dw_teams;         // 2: the depthwise warps form two teams of four that take alternate K-block steps, two 4x4 blocks per warp
@@ -324,20 +324,14 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                 const uint8_t* stage = smem + in_off + s * p.in_stage_stride;
                 // this K-block's depthwise taps + folded BN for the lane's channel pair (landed with the tile)
                 const uint8_t* prm = stage + p.in_stage_bytes;
-                const f32x2 sc = *reinterpret_cast<const f32x2*>(prm + KS * KS * 128 + lane * 8);        // (scale, scale) of the pair
-                const f32x2 bi = *reinterpret_cast<const f32x2*>(prm + KS * KS * 128 + 256 + lane * 8);  // (bias, bias)
+                constexpr int TAPS = dw_taps_bytes(KS);
+                const f32x2 sc = *reinterpret_cast<const f32x2*>(prm + TAPS + lane * 8);        // (scale, scale) of the pair
+                const f32x2 bi = *reinterpret_cast<const f32x2*>(prm + TAPS + 256 + lane * 8);  // (bias, bias)
                 // the A stage is normally free long before (deep ring): take it now so that every output row can be
                 // published the moment its last input row has been consumed -- the stores then drain during the math and
                 // the proxy fence at the end (a MEMBAR.ALL.CTA, ~36 cycles per store still in flight) finds few pending
                 mbar_wait_sel<kHint>(smem_u32(&bars->a_empty[sa]), pha ^ 1u);
                 uint8_t* a_s = smem + a_off + sa * TC_A_STAGE_BYTES;
-                constexpr bool kDwFfma2 = KS == 3;     // 3x3: taps widened to fp32 pairs once per step; 5x5: widened on use
-                // 5x5: the 25 tap words of the lane's channel pair, once per step (shared by both blocks of a team warp)
-                uint32_t wv[(HALFK || kDwFfma2) ? 1 : KS * KS];
-                if constexpr (!HALFK && !kDwFfma2) {
-#pragma unroll
-                    for (int i = 0; i < KS * KS; ++i) wv[i] = *reinterpret_cast<const uint32_t*>(prm + i * 128 + lane * 4);
-                }
 #pragma unroll 1
                 for (int blk = 0; blk < nblk; ++blk) {
                 const int bidx = member * nblk + blk;                      // 4x4-pixel block of the tile
@@ -347,8 +341,8 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                     static_assert(KS == 3 && STRIDE == 1, "half-K depthwise exists for the 3x3 stride-1 block only");
                     const int hl = lane & 15, hh = lane >> 4;       // channel pair, row half of the 4x4 block
                     const uint8_t* in_h = in_s - lane * 4 + hl * 4 + (hh * 2 * IW) * 128;
-                    const f32x2 sc2 = *reinterpret_cast<const f32x2*>(prm + KS * KS * 128 + hl * 8);
-                    const f32x2 bi2 = *reinterpret_cast<const f32x2*>(prm + KS * KS * 128 + 256 + hl * 8);
+                    const f32x2 sc2 = *reinterpret_cast<const f32x2*>(prm + TAPS + hl * 8);
+                    const f32x2 bi2 = *reinterpret_cast<const f32x2*>(prm + TAPS + 256 + hl * 8);
                     f32x2 acc[2][4];
 #pragma unroll
                     for (int a = 0; a < 2; ++a)
@@ -383,21 +377,27 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                             }
                         }
                     }
-                } else if constexpr (kDwFfma2) {
-                    // Every 16-bit word (the lane's channel pair) is widened to an fp32 pair once, then one fp32 FMA per
-                    // channel and pixel-tap.  A 16-bit x 16-bit product is exact in fp32, so this is the mixed-precision result.
+                } else {
+                    // Every 16-bit input word (the lane's channel pair) is widened to an fp32 pair once per row, then one fp32 FMA
+                    // per channel and pixel-tap.  A 16-bit x 16-bit product is exact in fp32, so this is the mixed-precision
+                    // result.  3x3: the 9 taps are widened once per step and stay in registers.  5x5: the taps are fp32 in the
+                    // parameter block and each (input row, output row) pair reads the lane's kernel row ky with three 16-byte
+                    // loads; holding all 25 would not fit beside the 32 accumulators and the row.
                     f32x2 acc[4][4];
 #pragma unroll
                     for (int a = 0; a < 4; ++a)
 #pragma unroll
                         for (int b = 0; b < 4; ++b) acc[a][b] = 0ull;
-                    f32x2 wq[KS][KS];
+                    constexpr bool kTapsInRegs = KS == 3;
+                    f32x2 wq[kTapsInRegs ? KS : 1][KS];
 #pragma unroll
                     for (int iy = 0; iy < IBH; ++iy) {
-                        if (iy < KS) {                                    // a kernel row is widened when its first input row arrives
+                        if constexpr (kTapsInRegs) {
+                            if (iy < KS) {                                // a kernel row is widened when its first input row arrives
 #pragma unroll
-                            for (int kx = 0; kx < KS; ++kx)
-                                wq[iy][kx] = MF::widen(*reinterpret_cast<const uint32_t*>(prm + (iy * KS + kx) * 128 + lane * 4));
+                                for (int kx = 0; kx < KS; ++kx)
+                                    wq[iy][kx] = MF::widen(*reinterpret_cast<const uint32_t*>(prm + (iy * KS + kx) * 128 + lane * 4));
+                            }
                         }
                         f32x2 row[IBW];
 #pragma unroll
@@ -406,47 +406,27 @@ block_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant
                         for (int oy = 0; oy < 4; ++oy) {
                             const int ky = iy - oy * STRIDE;
                             if (ky < 0 || ky >= KS) continue;
+                            f32x2 wk[KS];
+                            if constexpr (kTapsInRegs) {
+#pragma unroll
+                                for (int kx = 0; kx < KS; ++kx) wk[kx] = wq[ky][kx];
+                            } else {                                      // [5 rows][32 lanes][6 pairs], see dw_taps_bytes
+                                const uint8_t* tr = prm + (ky * 32 + lane) * 48;
+                                const uint4 t01 = lds_u4_here(tr), t23 = lds_u4_here(tr + 16), t4 = lds_u4_here(tr + 32);
+                                wk[0] = ((f32x2)t01.y << 32) | t01.x; wk[1] = ((f32x2)t01.w << 32) | t01.z;
+                                wk[2] = ((f32x2)t23.y << 32) | t23.x; wk[3] = ((f32x2)t23.w << 32) | t23.z;
+                                wk[4] = ((f32x2)t4.y << 32) | t4.x;
+                            }
 #pragma unroll
                             for (int ox = 0; ox < 4; ++ox)
 #pragma unroll
-                                for (int kx = 0; kx < KS; ++kx) ffma2(acc[oy][ox], row[ox * STRIDE + kx], wq[ky][kx]);
+                                for (int kx = 0; kx < KS; ++kx) ffma2(acc[oy][ox], row[ox * STRIDE + kx], wk[kx]);
                             if (ky == KS - 1) {                           // output row oy is complete: BN, act, pack, publish
 #pragma unroll
                                 for (int ox = 0; ox < 4; ++ox) {
                                     const int m = (ni * TH + br * 4 + oy) * TW + bc * 4 + ox;
                                     *reinterpret_cast<uint32_t*>(a_s + m * 128 + (((lane >> 2) ^ (m & 7)) << 4) + ((lane & 3) << 2)) =
                                         MF::template pack_act<RELU6>(ffma2_abc(acc[oy][ox], sc, bi));
-                                }
-                            }
-                        }
-                    }
-                } else {
-                    // 5x5: the 25 tap words stay packed (register budget); MixFma::fma2 widens on use
-                    float acc[4][4][2];
-#pragma unroll
-                    for (int a = 0; a < 4; ++a)
-#pragma unroll
-                        for (int b = 0; b < 4; ++b) acc[a][b][0] = acc[a][b][1] = 0.f;
-#pragma unroll
-                    for (int iy = 0; iy < IBH; ++iy) {
-                        uint32_t row[IBW];
-#pragma unroll
-                        for (int ix = 0; ix < IBW; ++ix) row[ix] = *reinterpret_cast<const uint32_t*>(in_s + (iy * IW + ix) * 128);
-#pragma unroll
-                        for (int oy = 0; oy < 4; ++oy) {
-                            const int ky = iy - oy * STRIDE;
-                            if (ky < 0 || ky >= KS) continue;
-#pragma unroll
-                            for (int ox = 0; ox < 4; ++ox)
-#pragma unroll
-                                for (int kx = 0; kx < KS; ++kx)
-                                    MF::fma2(acc[oy][ox][0], acc[oy][ox][1], row[ox * STRIDE + kx], wv[ky * KS + kx]);
-                            if (ky == KS - 1) {                           // output row oy is complete: BN, act, pack, publish
-#pragma unroll
-                                for (int ox = 0; ox < 4; ++ox) {
-                                    const int m = (ni * TH + br * 4 + oy) * TW + bc * 4 + ox;
-                                    *reinterpret_cast<uint32_t*>(a_s + m * 128 + (((lane >> 2) ^ (m & 7)) << 4) + ((lane & 3) << 2)) =
-                                        MF::template pack_act<RELU6>(ffma2_abc(f32x2_make(acc[oy][ox][0], acc[oy][ox][1]), sc, bi));
                                 }
                             }
                         }
@@ -882,7 +862,8 @@ void block_tc_destroy(BlockTcPlan* bp) {
     delete bp;
 }
 
-// per-K-block depthwise parameter block: [taps][64] 16-bit taps | [64] fp32 scale | [64] fp32 bias (zero padded)
+// per-K-block depthwise parameter block: taps | [64] fp32 scale | [64] fp32 bias (zero padded).  Taps are rounded to the storage
+// dtype; 3x3: kept in it as [9][64]; 5x5: widened exactly to fp32 as [5 rows][32 lanes][6 pairs] (see dw_taps_bytes).
 template <typename T>
 __global__ void pack_dwp_kernel(const float* __restrict__ w, const float* __restrict__ scale, const float* __restrict__ bias,
                                 uint8_t* __restrict__ dst, int taps, int c_in, int kblocks, int block_bytes, float post) {
@@ -890,10 +871,19 @@ __global__ void pack_dwp_kernel(const float* __restrict__ w, const float* __rest
     if (i >= kblocks * 64) return;
     const int kb = i / 64, cl = i % 64, c = kb * 64 + cl;
     uint8_t* blk = dst + (size_t)kb * block_bytes;
-    T* wt = reinterpret_cast<T*>(blk);
-    for (int t = 0; t < taps; ++t) wt[t * 64 + cl] = Traits<T>::from_f(c < c_in ? w[t * c_in + c] : 0.f);
-    reinterpret_cast<float*>(blk + taps * 128)[cl] = c < c_in ? scale[c] * post : 0.f;
-    reinterpret_cast<float*>(blk + taps * 128 + 256)[cl] = c < c_in ? bias[c] * post : 0.f;
+    for (int t = 0; t < taps; ++t) {
+        const T v = Traits<T>::from_f(c < c_in ? w[t * c_in + c] : 0.f);
+        if (taps == 25) {
+            float* row = reinterpret_cast<float*>(blk) + ((t / 5) * 32 + (cl >> 1)) * 12;    // kernel row t / 5 of lane cl / 2
+            row[(t % 5) * 2 + (cl & 1)] = Traits<T>::to_f(v);
+            if (t % 5 == 0) row[10 + (cl & 1)] = 0.f;
+        } else {
+            reinterpret_cast<T*>(blk)[t * 64 + cl] = v;
+        }
+    }
+    const int tb = taps == 25 ? dw_taps_bytes(5) : dw_taps_bytes(3);
+    reinterpret_cast<float*>(blk + tb)[cl] = c < c_in ? scale[c] * post : 0.f;
+    reinterpret_cast<float*>(blk + tb + 256)[cl] = c < c_in ? bias[c] * post : 0.f;
 }
 __global__ void pack_affine_kernel(const float* __restrict__ scale, const float* __restrict__ bias, float2* __restrict__ dst,
                                    int n_src, int n_dst, float post) {

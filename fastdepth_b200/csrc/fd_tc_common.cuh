@@ -282,6 +282,13 @@ __device__ __forceinline__ f32x2 ffma2_abc(f32x2 a, f32x2 b, f32x2 c) {
     return f32x2_make(fmaf(f32x2_lo(a), f32x2_lo(b), f32x2_lo(c)), fmaf(f32x2_hi(a), f32x2_hi(b), f32x2_hi(c)));
 }
 __device__ __forceinline__ void ffma2(f32x2& acc, f32x2 a, f32x2 b) { acc = ffma2_abc(a, b, acc); }
+// 16 bytes from shared memory, loaded where the call stands: the compiler neither hoists it nor merges it with an earlier load
+// of the same address, so it cannot decide to keep a whole tap table live in registers (and spill) to save the reloads
+__device__ __forceinline__ uint4 lds_u4_here(const void* p) {
+    uint4 v;
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(smem_u32(p)));
+    return v;
+}
 
 // mixed-precision FMA: exact 16-bit x 16-bit product added into fp32
 template <typename T> struct MixFma;
