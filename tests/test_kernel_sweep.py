@@ -3,7 +3,7 @@ against the per-stage fp64 interval reference (oracle/stage_ref.py) computed fro
 
 A 16-bit element must be a rounding of a value its interval admits, and exactly the round-to-nearest value wherever the
 interval holds no rounding midpoint (stage_ref.check); at least half of every single-stage 16-bit tensor must be
-determined that way (compositions through a chain run or a fused head: containment, see _check_plan).
+determined that way (compositions through a chain run or a fused head: containment, see plan_check.check_plan).
 The cases reach the kernel instances, activations, epilogues, cluster modes, channel tails and map edges that the two
 MobileNet networks of test_gpu_parity.py never execute.  Every case names the kernels it must run, and the last test
 asserts that the sweep as a whole covered every kernel variant."""
@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+import plan_check as pc
 from fastdepth_b200 import plan as fplan
 from oracle import stage_ref as sr
 
@@ -18,7 +19,6 @@ pytestmark = pytest.mark.gpu
 
 F16, BF16, F32 = torch.float16, torch.bfloat16, torch.float32
 R, R6 = sr.RELU, sr.RELU6
-MIN_DETERMINED = 0.5
 SEEN = []              # (kernel name, activation of its stage, dtype) of every step every case ran
 RAN = set()
 WORST = {}             # case id -> lowest determined fraction of its strictly checked tensors
@@ -152,29 +152,8 @@ def make_weights(descs, dtype, x, seed):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# running a case and checking it
+# running a case and checking it (tests/plan_check.py)
 # ---------------------------------------------------------------------------------------------------------------------
-def _nhwc(t, pick):
-    return t[pick].float().cpu().numpy().astype(np.float64)
-
-
-class Checker:
-    def __init__(self, case, dtype):
-        self.case, self.dtype, self.fracs = case, dtype, []
-        self.n = self.zeros = self.sixes = 0
-
-    def __call__(self, got, iv, what, strict=True):
-        self.n += got.size
-        self.zeros += int((got == 0).sum())
-        self.sixes += int((got == 6).sum())
-        f = sr.check(got, iv, self.dtype, '%s: %s' % (self.case, what))
-        if strict:
-            assert f >= MIN_DETERMINED, '%s: %s: only %.3f of the elements are determined' % (self.case, what, f)
-            self.fracs.append(f)
-        else:               # its determined elements are still held to exact equality by sr.check
-            COMPOSED[(self.case, what)] = f
-
-
 def run_case(case, descs, dtype, n, h, w, must=(), must_not=(), opts=None, env=None, seed=0, pick=None, x_fn=None,
              w_fn=None, monkeypatch=None, keep=False):
     opts = dict(opts or {})
@@ -198,46 +177,22 @@ def run_case(case, descs, dtype, n, h, w, must=(), must_not=(), opts=None, env=N
     x = torch.from_numpy(x_host).to(dtype).cuda()
     y = torch.empty((n, 1, h, w), dtype=dtype, device='cuda')
     stream = torch.cuda.current_stream().cuda_stream
-    has_add = any(d['skip_src'] >= 0 and not d['skip_mode'] for d in descs)
     inplace = opts.pop('inplace_skip', 1)
     for k, v in opts.items():
         p.set_option(k, v)
-    chk = Checker(case, dtype)
-    # pass 1: skip sources kept (inplace_skip 0) -- every materialised stage checked; pass 2: the in-place run's decoders
-    passes = [0, 1] if (has_add and inplace) else [inplace]
-    sources, kern = {}, ''
-    for ip in passes:
-        p.set_option('inplace_skip', ip)
-        p.forward(x, y, stream)
-        torch.cuda.synchronize()
-        steps = p.steps()
-        kern += ' ' + ' '.join(s['kernel'] for s in steps)
+    chk = pc.Checker(case, dtype)
+    # pass 1: skip sources kept (inplace_skip 0) -- every materialised stage checked; pass 2: the in-place run's decoders;
+    # then the chain's layers and the fused head on their own
+    ran = pc.check_plan(p, descs, weights, dtype, x_host, x, y, pick, chk, opts, inplace, stream)
+    kern = ' ' + ' '.join(s['kernel'] for steps in ran for s in steps)
+    for steps in ran:
         for s in steps:
             SEEN.append((s['kernel'], descs[s['stage']]['act'], dtype))
-        _check_plan(p, descs, weights, dtype, x_host, y, pick, steps, chk, sources, ip, ip and len(passes) == 2, opts)
     for m in must:
         assert m in kern, (case, m, kern)
     for m in must_not:
         assert m not in kern, (case, m, kern)
-    if 'chain_tc' in kern:
-        # the layers of every chain run one by one (per-block kernels), each checked from its own materialised input
-        p.set_option('chain', 0)
-        p.set_option('inplace_skip', 0)
-        p.forward(x, y, stream)
-        torch.cuda.synchronize()
-        _check_plan(p, descs, weights, dtype, x_host, y, pick, p.steps(), chk, {}, 0, False, dict(opts, chain=0))
-        p.set_option('chain', 1)
-    if '+head' in kern:
-        # the fused head on its own: the same plan with the head unfused materialises the last block's output (the same
-        # kernel instance and accumulation order), and the fused kernel's depth map is checked against the head of it
-        yf = y.clone()
-        p.set_option('fold_head', 0)
-        p.set_option('inplace_skip', 0)
-        p.forward(x, y, stream)
-        torch.cuda.synchronize()
-        _check_plan(p, descs, weights, dtype, x_host, y, pick, p.steps(), chk, {}, 0, False, dict(opts, fold_head=0))
-        last = sr.exact(_nhwc(p.stage_tensor(len(descs) - 2), pick))
-        chk(_nhwc(yf[:, 0], pick), sr.head(last, *weights[-1][3:], descs[-1]['act']), 'fused head')
+    COMPOSED.update({(case, what): f for what, f in chk.composed.items()})
     # the activations are live: not mostly zeros, and ReLU6 really clamps somewhere
     assert chk.zeros < 0.5 * chk.n, (case, chk.zeros / chk.n)
     if any(d['act'] == R6 for d in descs[:-1]):
@@ -248,102 +203,6 @@ def run_case(case, descs, dtype, n, h, w, must=(), must_not=(), opts=None, env=N
         return p, x, y
     p.close()
     return y
-
-
-def _check_plan(p, descs, weights, dtype, x_host, y, pick, steps, chk, sources, ip, recheck, opts):
-    """Check every stage the plan materialised (``recheck``: only the decoder blocks that add in place, and the head)."""
-    ns = len(descs)
-    q = None if dtype == F32 else dtype
-    fold = opts.get('fold_head', 1) and descs[-2]['upsample'] and descs[-2]['skip_src'] < 0
-    chained = {}                                   # first stage of a chain run -> last stage
-    for s in steps:
-        if 'chain_tc' in s['kernel']:
-            a, b = s['kernel'].split('{stages ')[1].rstrip('}').split('-')
-            chained[int(a)] = int(b)
-    head_fused = any('+head' in s['kernel'] for s in steps)
-    path0 = opts.get('path', 1) == 0
-    is_src = {d['skip_src'] for d in descs if d['skip_src'] >= 0 and not d['skip_mode']}
-
-    def buf(i):
-        return sr.exact(_nhwc(p.stage_tensor(i), pick))
-
-    def stage_input(i):
-        if i == 0:
-            return None
-        d = descs[i - 1]
-        t = buf(i - 1)
-        if d['skip_src'] >= 0 and d['skip_mode']:
-            t = sr.concat(t, buf(d['skip_src']))
-        return t
-
-    def skip_of(d):
-        src = d['skip_src']
-        if src < 0 or d['skip_mode']:
-            return None
-        return sources[src] if ip else buf(src)
-
-    i = 0
-    while i < ns - 1:
-        d = descs[i]
-        if d['kind'] == sr.STEM:
-            if not recheck:
-                chk(_nhwc(p.stage_tensor(0), pick),
-                    sr.stem(x_host[pick], weights[0][3], weights[0][4], weights[0][5], d['stride'], d['act']), 'stem')
-                if 0 in is_src:
-                    sources[0] = buf(0)
-            i += 1
-            continue
-        last = i == ns - 2
-        if recheck and not (d['skip_src'] >= 0 and not d['skip_mode']):
-            i += 1
-            continue
-        if i in chained:                           # a run inside one chain kernel: composition from the run's input
-            j = chained[i]
-            cur = stage_input(i)
-            for t in range(i, j + 1):
-                r = sr.dwpw(cur, weights[t], descs[t], q)['out']
-                cur = sr.quantize(r, q) if t < j else r
-            # containment only: over several layers the worst-case radii of the intermediate rounding flips outgrow the ulp;
-            # run_case holds every one of these layers to the full rule in the same plan without the chain kernel
-            chk(_nhwc(p.stage_tensor(j), pick), cur, 'chain %d-%d' % (i, j), strict=False)
-            if j in is_src:
-                sources[j] = buf(j)
-            i = j + 1
-            continue
-        if last and head_fused:                    # block + head in one kernel: composition from the block's input
-            r = sr.dwpw(stage_input(i), weights[i], dict(d, upsample=0), q)['out']
-            hd = sr.head(sr.quantize(r, q), *weights[-1][3:], descs[-1]['act'])
-            # a composition through a whole block: the worst-case radii of the rounding flips inside the block add up over the
-            # head's dot product, so only containment is demanded here; the fused head is held to the determined-fraction rule
-            # against the unfused plan in run_case
-            chk(_nhwc(y[:, 0], pick), sr.upsample(hd), 'block %d + head' % i, strict=False)
-            return
-        dd = dict(d, upsample=0) if (last and fold) else d
-        r = sr.dwpw(stage_input(i), weights[i], dd, q, skip_of(d))
-        if path0:                                  # both halves on their own, from the kernel's own intermediate
-            chk(_nhwc(p.stage_tensor(i, which=1), pick), r['dw'], 'stage %d depthwise' % i)
-            mid = sr.exact(_nhwc(p.stage_tensor(i, which=1), pick))
-            r = _pw_from_mid(mid, weights[i], dd, q, skip_of(d))
-        chk(_nhwc(p.stage_tensor(i), pick), r['out'], 'stage %d' % i)
-        if i in is_src and not ip:
-            sources[i] = buf(i)
-        i += 1
-    if head_fused:
-        return                                     # (checked in the first pass)
-    # the head (unfused): from the last block's buffer
-    hin = stage_input(ns - 1)
-    hd = sr.head(hin, *weights[-1][3:], descs[-1]['act'])
-    chk(_nhwc(y[:, 0], pick), sr.upsample(hd) if fold else hd, 'head')
-
-
-def _pw_from_mid(mid, wt, d, q, skip):
-    p = sr.pointwise(mid, wt[3], wt[4], wt[5], d['act'])
-    out = p
-    if d['upsample']:
-        out = sr.upsample(p)
-        if skip is not None and not d['skip_mode']:
-            out = sr.add(sr.quantize(out, q), skip)
-    return {'pw': p, 'out': out}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
