@@ -14,6 +14,7 @@ namespace fd {
 
 BlockPlanOut block_tc_debug_plan(int ksize, int stride, int h_out, int w_out, int n, int c_in, int c_out, int head);
 ConvPlanOut conv_tc_debug_plan(int kind, int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms);
+ConvPlanOut pw_tf32x3_debug_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms);
 
 // ---- error state -----------------------------------------------------------------------
 static thread_local std::string g_last_error;
@@ -70,6 +71,10 @@ int conv_tc_prepare(int dtype, int kind, const StageGeom& g, const void* in, con
 int conv_tc_launch(ConvTcPlan* cp, cudaStream_t st);
 void conv_tc_destroy(ConvTcPlan* cp);
 const char* conv_tc_name(ConvTcPlan* cp);
+// the split-TF32 pointwise step of an fp32 DWPW stage (fd_conv_tc.cu)
+bool pw_tf32x3_supported(const StageGeom& g);
+int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w, const float* scale_dev, const float* bias_dev,
+                      void* out, int out_pitch, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res);
 
 static size_t dtype_size(int dtype) { return dtype == FD_F32 ? 4 : 2; }
 static bool is_phased(int kind) { return kind == FD_STAGE_DECONV || kind == FD_STAGE_UPCONV; }
@@ -123,6 +128,7 @@ struct fd_plan {
     int opt_path = 1, opt_fold_head = 1, opt_graph = 1, opt_tma_epilogue = 1, opt_inplace_skip = 1, opt_pdl = 0, opt_wait_sleep_ns = 0;
     int opt_chain = 1;
     int opt_cluster = 1;
+    int opt_tf32x3 = 0;
     size_t workspace_bytes = 0;
     // fd_pipeline_*: host batches flow H2D -> forward -> D2H through kPipeSlots device slots on three streams
     struct PipeSlot { void* x = nullptr; void* y = nullptr; cudaEvent_t up = nullptr, done = nullptr, down = nullptr; bool busy = false; };
@@ -391,7 +397,32 @@ static int build_steps(fd_plan* p) {
                 q.macs = pw_macs;
                 q.alg_bytes = (px_out * s.g.c_in + px_out * up * s.g.c_out * (a.skip ? 2.0 : 1.0)) * es +
                               (double)s.g.c_in * s.g.c_out * es + 2.0 * s.g.c_out * 4;
-                q.run = [a, dtype](cudaStream_t stream, const void*, void*) { return launch_pw(dtype, a, stream); };
+                if (dtype == FD_F32 && p->opt_path == 1 && p->opt_tf32x3 && pw_tf32x3_supported(a.g)) {
+                    // the pointwise half as split TF32 on wgmma (conv_tc_tf32x3_kernel).  A skip is added by a TMA reduce-add
+                    // of the tiles: into the skip tensor itself (inplace_skip, which then becomes the stage output), or into
+                    // the stage's own buffer after a device copy of the skip; either way the result is skip + up rounded once
+                    const bool add = a.skip != nullptr;
+                    const bool inplace = add && p->opt_inplace_skip;
+                    void* out = inplace ? const_cast<void*>(a.skip) : a.out;
+                    const int opitch = inplace ? a.g.skip_pitch : a.g.out_pitch;
+                    if (inplace) s.out_eff = out;
+                    int rc = pw_tf32x3_prepare(a.g, a.mid, static_cast<const float*>(a.pw_w), a.pw_scale, a.pw_bias, out, opitch,
+                                               add ? 1 : 0, lopts, &s.ctc);
+                    if (rc != FD_OK) return rc;
+                    q.name = conv_tc_name(s.ctc);
+                    ConvTcPlan* ctc = s.ctc;
+                    const bool copy = add && !inplace;
+                    const void* skip = a.skip;
+                    const size_t rows = (size_t)a.g.n * s.out_h * s.out_w, row_bytes = (size_t)a.g.c_out * 4;
+                    const size_t dpitch = (size_t)a.g.out_pitch * 4, spitch = (size_t)a.g.skip_pitch * 4;
+                    q.run = [ctc, copy, out, skip, rows, row_bytes, dpitch, spitch](cudaStream_t stream, const void*, void*) {
+                        if (copy)
+                            FD_CUDA_OK(cudaMemcpy2DAsync(out, dpitch, skip, spitch, row_bytes, rows, cudaMemcpyDeviceToDevice, stream));
+                        return conv_tc_launch(ctc, stream);
+                    };
+                } else {
+                    q.run = [a, dtype](cudaStream_t stream, const void*, void*) { return launch_pw(dtype, a, stream); };
+                }
                 p->steps.push_back(q);
             }
         } else if (!head_fused) {  // HEAD (unless decode_conv6 already ran inside the last block's epilogue)
@@ -632,6 +663,7 @@ static int* option_slot(fd_plan* p, const char* name) {
     if (!strcmp(name, "wait_sleep_ns")) return &p->opt_wait_sleep_ns;
     if (!strcmp(name, "chain")) return &p->opt_chain;
     if (!strcmp(name, "cluster")) return &p->opt_cluster;
+    if (!strcmp(name, "tf32x3")) return &p->opt_tf32x3;
     return nullptr;
 }
 
@@ -935,6 +967,15 @@ int fd_debug_conv_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_o
     const ConvPlanOut q = conv_tc_debug_plan(FD_STAGE_CONV, ksize, h_out, w_out, n, c_in, c_out, n_sms);
     const int v[16] = {q.ok, q.ni, q.th, q.tw, q.bn, q.stages, q.m_tiles, q.n_splits, q.items, q.waves, q.kblocks, q.smem_bytes,
                        q.useful_permille, (int)(q.cost > 2e9 ? 2e9 : q.cost), 0, 0};
+    for (int i = 0; i < 16; ++i) out[i] = v[i];
+    return FD_OK;
+}
+
+int fd_debug_pw_tf32x3_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms, int* out, int cap) {
+    if (!out || cap < 16) return fail(FD_ERR_INVALID, "need an int[16] output");
+    const ConvPlanOut q = pw_tf32x3_debug_plan(h_out, w_out, n, c_in, c_out, upsample, n_sms);
+    const int v[16] = {q.ok, q.ni, q.th, q.tw, q.bn, q.stages, q.m_tiles, q.n_splits, q.items, q.waves, q.kblocks, q.smem_bytes,
+                       q.useful_permille, (int)(q.cost > 2e9 ? 2e9 : q.cost), q.ok ? conv_stage_bytes_tf32x3(q.bn) : 0, 0};
     for (int i = 0; i < 16; ++i) out[i] = v[i];
     return FD_OK;
 }

@@ -15,6 +15,12 @@
 // differ in cost (9 / 6 / 6 / 4 taps for k = 5), so an item is (tile, bn split, phase group): either one phase per item or the
 // two diagonal pairs {00, 11} and {01, 10}.  Items are ordered group-major, heaviest group first, and the cost model takes the
 // makespan of the persistent grid's static round-robin assignment over the real per-item tap counts.
+//
+// The split-TF32 pointwise instance (tf32x3: an fp32 1x1 conv as three TF32 products per term, fd_conv_tc.cu) has an fp32
+// operand format: one 128-byte row holds 32 fp32 channels, so a K-block is 32 channels, and a stage holds the A box (16 KB)
+// plus two B boxes, the weights' TF32 high and low parts (2 x bn x 128 B).  Its MMA time counts three TF32 products per MAC
+// at the dense TF32 rate (1024 MAC / clock / SM, half the 16-bit rate); the consumers read A with ordinary shared loads (to
+// split it in registers) and every wgmma reads one of the two B boxes; the fp32 output tile is twice as many bytes.
 #pragma once
 
 namespace fd {
@@ -74,6 +80,7 @@ struct ConvPlanIn {
     int force_tile;            // -1 = the cost model chooses, else an index into kConvTiles
     int kind;                  // kConvKind*; 0 = CONV
     int force_group;           // phases per item of a DECONV / UPCONV stage: 0 = the cost model chooses, 1 = one, 2 = pairs
+    int tf32x3;                // 1: the split-TF32 pointwise instance (fp32 operands, 1x1 CONV only)
 };
 struct ConvPlanOut {
     int ok;
@@ -91,6 +98,11 @@ constexpr int kConvTiles[][3] = {{1, 8, 16}, {2, 8, 8}, {4, 4, 8}, {8, 4, 4}, {3
 constexpr int kConvNumTiles = 5;
 
 inline int conv_stage_bytes(int bn) { return 128 * 128 + bn * 128; }
+// the split-TF32 pointwise instance: A {32 fp32 ch x 128 px} + B high + B low {32 fp32 ch x bn}
+inline int conv_stage_bytes_tf32x3(int bn) { return 128 * 128 + 2 * bn * 128; }
+// bn 256 is not offered: 128 accumulators plus the 32 registers of a stage's split A fragments exceed the 168 registers a
+// thread of the 288-thread CTA may hold (ptxas serialises the wgmmas and spills)
+constexpr int kConvTf32x3MaxBn = 128;
 
 inline ConvPlanOut plan_conv_one(const ConvPlanIn& q, int tile, int bn, int per_item) {
     ConvPlanOut o{};
@@ -116,25 +128,32 @@ inline ConvPlanOut plan_conv_one(const ConvPlanIn& q, int tile, int bn, int per_
     const int ni = kConvTiles[tile][0], th = kConvTiles[tile][1], tw = kConvTiles[tile][2];
     const int sms = q.n_sms > 0 ? q.n_sms : 132;
     o.ni = ni; o.th = th; o.tw = tw; o.bn = bn;
-    o.kblocks = (q.c_in + 63) / 64;
+    const int kb_ch = q.tf32x3 ? 32 : 64;             // channels per 128-byte row
+    o.kblocks = (q.c_in + kb_ch - 1) / kb_ch;
     o.m_tiles = ((q.n + ni - 1) / ni) * ((q.h_out + th - 1) / th) * ((q.w_out + tw - 1) / tw);
     o.n_splits = (q.c_out + bn - 1) / bn;
     o.items = o.m_tiles * o.n_splits * o.groups;
     o.waves = (o.items + sms - 1) / sms;
     const int fixed = 2 * kConvStg + kConvBarrierBytes + kConvAlignSlack;
-    o.stages = (kConvSmemBudget - fixed) / conv_stage_bytes(bn);
+    const int stage_bytes = q.tf32x3 ? conv_stage_bytes_tf32x3(bn) : conv_stage_bytes(bn);
+    o.stages = (kConvSmemBudget - fixed) / stage_bytes;
     if (o.stages > kConvMaxStages) o.stages = kConvMaxStages;
-    o.smem_bytes = fixed + o.stages * conv_stage_bytes(bn);
+    o.smem_bytes = fixed + o.stages * stage_bytes;
     const double px = (double)q.n * q.h_out * q.w_out;
     o.useful_permille = (int)(1000.0 * px / ((double)o.m_tiles * 128.0));
     o.ok = o.stages >= 2 && o.smem_bytes <= kConvSmemBudget && o.kblocks > 0 && o.items > 0;
     // cost of one item in clocks (see the header comment), times the waves of the persistent launch
-    const double mma = 4.0 * bn, smem_rd = (2.0 * 8192 + 2.0 * bn * 128) / 128.0, l2 = (16384.0 + 128.0 * bn) / 40.0;
+    double mma = 4.0 * bn, smem_rd = (2.0 * 8192 + 2.0 * bn * 128) / 128.0, l2 = (16384.0 + 128.0 * bn) / 40.0;
+    if (q.tf32x3) {                                   // 3 TF32 products of 128 x bn x 32 MACs; A by shared loads, B read by 3 wgmmas
+        mma = 3.0 * 128.0 * bn * 32.0 / 1024.0;
+        smem_rd = (16384.0 + 2.0 * 3.0 * bn * 128) / 128.0;
+        l2 = (16384.0 + 256.0 * bn) / 40.0;
+    }
     double kstep = mma;
     if (smem_rd > kstep) kstep = smem_rd;
     if (l2 > kstep) kstep = l2;
     kstep += 40.0;                                    // barrier hand-shakes per K-block
-    const double epi = 128.0 * bn * 2.0 * (q.upsample ? 4.0 : 1.0) / 64.0 + 500.0;
+    const double epi = 128.0 * bn * (q.tf32x3 ? 4.0 : 2.0) * (q.upsample ? 4.0 : 1.0) / 64.0 + 500.0;
     // makespan of the static round-robin: CTA b of G runs items b, b + G, ...; group g holds items [g * per, (g + 1) * per)
     const int G = o.items < sms ? o.items : sms, per = o.m_tiles * o.n_splits;
     double gcost[4] = {0.0, 0.0, 0.0, 0.0};
@@ -162,6 +181,7 @@ inline ConvPlanOut plan_conv(const ConvPlanIn& q) {
     const bool phased = q.kind == kConvKindDeconv || q.kind == kConvKindUpconv;
     if (q.force_group && (!phased || q.force_group > 2)) return best;
     if (phased && (q.ksize < 3 || q.ksize > 9 || !(q.ksize & 1))) return best;
+    if (q.tf32x3 && (phased || q.ksize != 1)) return best;
     if (q.ksize < 1 || q.h_out < 1 || q.w_out < 1 || q.n < 1 || q.c_in < 8 || q.c_out < 8) return best;
     const int bns[3] = {64, 128, 256};
     for (int t = 0; t < kConvNumTiles; ++t) {
@@ -169,6 +189,7 @@ inline ConvPlanOut plan_conv(const ConvPlanIn& q) {
         for (int b = 0; b < 3; ++b) {
             const int bn = bns[b];
             if (q.force_bn ? bn != q.force_bn : (b > 0 && bn / 2 >= q.c_out)) continue;   // no split wider than twice the need
+            if (q.tf32x3 && bn > kConvTf32x3MaxBn) continue;
             for (int per_item = 1; per_item <= 2; ++per_item) {
                 if (q.force_group ? per_item != q.force_group : (per_item == 2 && (q.kind == 0 || q.kind == kConvKindConv)))
                     continue;

@@ -18,6 +18,17 @@
 // input resolution (fd_conv_plan.h): an item is then (tile, bn split, phase group); the producer's box loop and the
 // consumers' K loop come from the phase's {tap0, ny, nx, dy0, dx0}, and phase 2 ry + rx is stored through output view
 // tm_o[2 ry + rx] (the same four strided views as the upsample).  A CONV stage is one phase, the k x k square.
+//
+// conv_tc_tf32x3_kernel is the fp32 pointwise (1x1) conv of a DWPW stage as split TF32 (plan option "tf32x3"): the same
+// item decode, persistent item loop, operand ring and output views, with fp32 operands.  A K-block is 32 fp32 channels (one
+// 128-byte row); a stage is the A box {32 ch, tw, th, ni} of the depthwise intermediate plus two B boxes {32 ch, bn rows}, the
+// weights' TF32 high and low parts (split once when the plan is built).  The consumers split A themselves: each thread loads
+// its wgmma A fragment from the swizzled tile, rounds it to a_hi = rna(a), a_lo = rna(a - a_hi), and per k8 step issues
+// a_lo b_hi, a_hi b_lo, a_hi b_hi (small terms first) into one fp32 accumulator, A from registers.  The epilogue applies the
+// BN affine and act in fp32 and stores [128 px][32 ch] fp32 tiles; a skip add is a TMA reduce-add (.add.f32) of that tile
+// into the skip tensor (or a copy of it), so the stage output is skip + up rounded once.  It is a sibling kernel rather
+// than an instance of conv_tc_kernel: producer, K loop and epilogue all differ (two B boxes, A through registers, three
+// MMAs per step, fp32 stores or reduce-adds), and the 16-bit instances stay exactly as they were.
 #include <cstdio>
 #include <cstring>
 #include <new>
@@ -193,6 +204,136 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
     }
 }
 
+template <int BN, bool RELU6>
+__global__ void __launch_bounds__(CV_THREADS, 1)
+conv_tc_tf32x3_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
+                      const __grid_constant__ CUtensorMap tm_o0, const __grid_constant__ CUtensorMap tm_o1,
+                      const __grid_constant__ CUtensorMap tm_o2, const __grid_constant__ CUtensorMap tm_o3,
+                      const __grid_constant__ ConvParams p, const int reduce) {
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
+    // carve-up: [stages x (A 16 KB | B high bn x 128 B | B low bn x 128 B)][2 staging tiles][barriers]
+    const uint32_t stg_off = (uint32_t)p.stages * (uint32_t)p.stage_bytes;
+    const uint32_t bar_off = stg_off + 2u * (uint32_t)kConvStg;
+    ConvBarriers* bars = reinterpret_cast<ConvBarriers*>(smem + bar_off);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+    if (threadIdx.x == 0) {
+        // a stage is released by every consumer warp: each one reads its A fragment with its own shared loads
+        for (int i = 0; i < kConvMaxStages; ++i) { mbar_init(smem_u32(&bars->full[i]), 1); mbar_init(smem_u32(&bars->empty[i]), 8); }
+        fence_barrier_init();
+    }
+    if (warp == CV_WARP_TMA && lane == 0) {
+        tma_prefetch_desc(&tm_in); tma_prefetch_desc(&tm_w); tma_prefetch_desc(&tm_o0);
+        if (p.upsample) { tma_prefetch_desc(&tm_o1); tma_prefetch_desc(&tm_o2); tma_prefetch_desc(&tm_o3); }
+    }
+    pdl_launch_dependents();
+    pdl_wait_prior_grid();
+    __syncthreads();
+
+    if (warp == CV_WARP_TMA) {
+        // =========================== TMA producer ===========================
+        if (lane == 0) {
+            Ring r;
+            for (int w = blockIdx.x; w < p.items; w += gridDim.x) {
+                const ConvCoord c = conv_decode(p, w, BN);
+                for (int kb = 0; kb < p.kblocks; ++kb, r.next((uint32_t)p.stages)) {
+                    const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes, bar = smem_u32(&bars->full[r.s]);
+                    mbar_wait(smem_u32(&bars->empty[r.s]), r.ph ^ 1u);
+                    mbar_expect_tx(bar, (uint32_t)p.stage_bytes);
+                    tma_load_4d(st, &tm_in, bar, kb * 32, c.ox0, c.oy0, c.img0);
+                    tma_load_3d(st + CV_A_BYTES, &tm_w, bar, kb * 32, c.n0, 0);                  // high part
+                    tma_load_3d(st + CV_A_BYTES + BN * 128, &tm_w, bar, kb * 32, c.n0, 1);       // low part
+                }
+            }
+        }
+    } else {
+        // =========================== consumer warpgroups: split + wgmma + epilogue ===========================
+        const int wg = warp >> 2, wq = warp & 3;
+        const int r0 = wg * 64 + wq * 16 + (lane >> 2), cq = (lane & 3) * 2, t = lane & 3;
+        const uint32_t sw = (uint32_t)(lane >> 2);     // r0 & 7 == (r0 + 8) & 7: the row's 16-byte chunk swizzle
+        const bool releaser = lane == 0;
+        const bool elected = warp == 0 && lane == 0;
+        constexpr uint32_t bar_id = 1u, bar_n = 256u;
+        Ring r;
+        uint32_t stg_flip = 0;
+        for (int w = blockIdx.x; w < p.items; w += gridDim.x) {
+            const ConvCoord c = conv_decode(p, w, BN);
+            float acc[BN / 2];
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            for (int k = 0; k < p.kblocks; ++k) {
+                mbar_wait(smem_u32(&bars->full[r.s]), r.ph);
+                const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes;
+                const uint8_t* a_tile = smem + r.s * (uint32_t)p.stage_bytes;
+                // this thread's A fragments of the four k8 steps: channel 8 k4 + t (+ 4) of rows r0 and r0 + 8, split
+                uint32_t a_hi[4][4], a_lo[4][4];
+#pragma unroll
+                for (int k4 = 0; k4 < 4; ++k4)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int row = r0 + (e & 1) * 8, ch = 8 * k4 + t + (e >> 1) * 4;
+                        const float v = *reinterpret_cast<const float*>(a_tile + row * 128 + ((((uint32_t)ch >> 2) ^ sw) << 4) + (ch & 3) * 4);
+                        a_hi[k4][e] = rna_tf32(v);
+                        a_lo[k4][e] = rna_tf32(v - __uint_as_float(a_hi[k4][e]));
+                    }
+                const uint32_t bh = sw128_desc_lo(st + CV_A_BYTES), bl = sw128_desc_lo(st + CV_A_BYTES + BN * 128);
+                wgmma_fence();
+#pragma unroll
+                for (int k4 = 0; k4 < 4; ++k4) {               // +32 B (8 fp32 channels) per k8 step inside the 128-byte row
+                    wgmma_tf32_bn<BN>(acc, a_lo[k4], sw128_desc(bh + 2u * k4), (k > 0 || k4 > 0) ? 1u : 0u);
+                    wgmma_tf32_bn<BN>(acc, a_hi[k4], sw128_desc(bl + 2u * k4), 1u);
+                    wgmma_tf32_bn<BN>(acc, a_hi[k4], sw128_desc(bh + 2u * k4), 1u);
+                }
+                wgmma_commit();
+                // the A registers are rewritten by the next step: wait for this step's MMAs, then release the stage
+                wgmma_wait0();
+                if (releaser) mbar_arrive(smem_u32(&bars->empty[r.s]));
+                r.next((uint32_t)p.stages);
+            }
+
+            // per block of 32 output channels: registers -> BN affine + act (fp32) -> staging tile [128 px][32 ch] fp32
+            // (16-byte chunks XOR-swizzled like a SWIZZLE_128B box) -> TMA tensor stores or reduce-adds
+#pragma unroll
+            for (int cb = 0; cb < BN / 32; ++cb) {
+                if (c.n0 + cb * 32 >= p.c_out) break;
+                uint8_t* stg = smem + stg_off + (stg_flip & 1u) * (uint32_t)kConvStg;
+                ++stg_flip;
+                const float2* aff = p.affine + c.n0 + cb * 32;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {                  // 8-column group i of this block
+                    const float4 af = __ldg(reinterpret_cast<const float4*>(aff + i * 8 + cq));     // (s0, s1, b0, b1)
+                    const int j = cb * 4 + i, cl = i * 8 + cq;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int rr = r0 + 8 * h;
+                        float v0 = fmaxf(fmaf(acc[4 * j + 2 * h], af.x, af.z), 0.0f);
+                        float v1 = fmaxf(fmaf(acc[4 * j + 2 * h + 1], af.y, af.w), 0.0f);
+                        if (RELU6) { v0 = fminf(v0, 6.0f); v1 = fminf(v1, 6.0f); }
+                        *reinterpret_cast<float2*>(stg + rr * 128 + ((((uint32_t)cl >> 2) ^ sw) << 4) + (cl & 3) * 4) = make_float2(v0, v1);
+                    }
+                }
+                fence_proxy_async();
+                if (elected) bulk_wait_read0();
+                asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");
+                if (elected) {
+                    const uint32_t src = smem_u32(stg);
+                    const int cc = c.n0 + cb * 32;
+                    const int nv = p.upsample ? 4 : 1;
+                    for (int v = 0; v < nv; ++v) {
+                        const CUtensorMap* m = v == 0 ? &tm_o0 : v == 1 ? &tm_o1 : v == 2 ? &tm_o2 : &tm_o3;
+                        if (reduce) tma_reduce_add_4d(m, src, cc, c.ox0, c.oy0, c.img0);
+                        else tma_store_4d(m, src, cc, c.ox0, c.oy0, c.img0);
+                    }
+                    bulk_commit_group();
+                }
+            }
+        }
+        if (elected) bulk_wait_all();
+    }
+}
+
 // ----------------------------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------------------------
@@ -205,8 +346,21 @@ struct ConvTcPlan {
     int dtype, act;
     TcLaunchOpts opts;
     float2* affine = nullptr;
+    float* w_split = nullptr;            // tf32x3: [2][c_out][c_in] fp32, the weights' TF32 high then low parts
+    int tf32x3 = 0, reduce = 0;
     std::string name;
 };
+
+// w_hi = rna_tf32(w), w_lo = rna_tf32(w - w_hi) (w - w_hi is exact in fp32)
+__global__ void split_tf32_kernel(const float* __restrict__ w, float* __restrict__ dst, int count) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < count) {
+        const float v = w[i];
+        const float hi = __uint_as_float(rna_tf32(v));
+        dst[i] = hi;
+        dst[count + i] = __uint_as_float(rna_tf32(v - hi));
+    }
+}
 
 __global__ void pack_conv_affine_kernel(const float* __restrict__ scale, const float* __restrict__ bias, float2* __restrict__ dst,
                                         int c_out, int n_pad) {
@@ -229,6 +383,7 @@ bool conv_tc_supported(int dtype, const StageGeom& g, int kind) {
 void conv_tc_destroy(ConvTcPlan* cp) {
     if (!cp) return;
     cudaFree(cp->affine);
+    cudaFree(cp->w_split);
     delete cp;
 }
 
@@ -336,6 +491,105 @@ int conv_tc_prepare(int dtype, int kind, const StageGeom& g, const void* in, con
     return FD_OK;
 }
 
+bool pw_tf32x3_supported(const StageGeom& g) {
+    return g.c_in % 8 == 0 && g.c_out % 8 == 0 && get_tensor_map_encoder() != nullptr;
+}
+
+ConvPlanOut pw_tf32x3_debug_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms) {
+    ConvPlanIn q{};
+    q.ksize = 1; q.h_out = h_out; q.w_out = w_out; q.n = n; q.c_in = c_in; q.c_out = c_out; q.upsample = upsample;
+    q.n_sms = n_sms; q.force_tile = -1; q.kind = kConvKindConv; q.tf32x3 = 1;
+    return plan_conv(q);
+}
+
+// The split-TF32 pointwise step of an fp32 DWPW stage: `mid` is the stage's depthwise intermediate (NHWC fp32, c_in dense),
+// `w` its fp32 pointwise weights [c_out][c_in], `out` / `out_pitch` what the tiles are written to (g.upsample: through the
+// four views of the 2x map).  reduce = 1: the tiles are reduce-added into `out`, which already holds the skip tensor.
+// FD_CONV_TILE / FD_CONV_BN pin the planner's choice as for conv_tc_prepare.
+int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w, const float* scale_dev, const float* bias_dev,
+                      void* out, int out_pitch, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res) {
+    PFN_encodeTiled encode = get_tensor_map_encoder();
+    if (!encode) return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    ConvPlanIn q{};
+    q.ksize = 1; q.h_out = g.h_out; q.w_out = g.w_out; q.n = g.n; q.c_in = g.c_in; q.c_out = g.c_out; q.upsample = g.upsample;
+    q.n_sms = opts.n_sms; q.force_tile = -1; q.kind = kConvKindConv; q.tf32x3 = 1;
+    { const char* e = getenv("FD_CONV_TILE"); if (e && *e) q.force_tile = atoi(e); }
+    { const char* e = getenv("FD_CONV_BN"); if (e && *e) q.force_bn = atoi(e); }
+    const ConvPlanOut po = plan_conv(q);
+    if (!po.ok) return fail(FD_ERR_UNSUPPORTED, "tf32x3 pointwise step: no tile plan fits shared memory");
+    ConvTcPlan* cp = new (std::nothrow) ConvTcPlan();
+    if (!cp) return fail(FD_ERR_CUDA, "out of host memory");
+    cp->dtype = FD_F32; cp->act = g.act; cp->opts = opts; cp->po = po; cp->tf32x3 = 1; cp->reduce = reduce;
+    ConvParams& p = cp->p;
+    memset(&p, 0, sizeof(p));
+    p.n = g.n; p.h = g.h_out; p.w = g.w_out; p.c_in = g.c_in; p.c_out = g.c_out;
+    p.ni = po.ni; p.th = po.th; p.tw = po.tw;
+    p.tiles_x = (g.w_out + po.tw - 1) / po.tw; p.tiles_y = (g.h_out + po.th - 1) / po.th; p.img_tiles = (g.n + po.ni - 1) / po.ni;
+    p.splits = po.n_splits; p.items = po.items;
+    p.kblocks = po.kblocks;
+    p.stages = po.stages; p.stage_bytes = conv_stage_bytes_tf32x3(po.bn);
+    p.upsample = g.upsample;
+    memcpy(p.ph, po.ph, sizeof(p.ph));
+    for (int i = 0; i < 4; ++i) p.group_code[i] = 0xF;
+    p.group_code[0] = 0xF0;                        // one group: phase 0, the 1x1 "square"
+    auto magic = [](int d) { return (unsigned long long)((1ULL << 40) / (unsigned long long)d) + 1ULL; };
+    p.mg_splits = magic(p.splits); p.mg_tx = magic(p.tiles_x); p.mg_ty = magic(p.tiles_y); p.mg_img = magic(p.img_tiles);
+    const int n_pad = p.splits * po.bn;
+    const int wcount = g.c_in * g.c_out;
+    if (cudaMalloc(&cp->affine, (size_t)n_pad * sizeof(float2)) != cudaSuccess ||
+        cudaMalloc(&cp->w_split, (size_t)2 * wcount * sizeof(float)) != cudaSuccess) {
+        conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cudaMalloc failed"); }
+    pack_conv_affine_kernel<<<(n_pad + 127) / 128, 128>>>(scale_dev, bias_dev, cp->affine, g.c_out, n_pad);
+    split_tf32_kernel<<<(wcount + 255) / 256, 256>>>(w, cp->w_split, wcount);
+    if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "tf32x3 weight packing failed"); }
+    p.affine = cp->affine;
+
+    const size_t es = 4;
+    const CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    {   // depthwise intermediate: NHWC (C, W, H, N), box (32, tw, th, ni); OOB -> 0 (the channel tail of the last K-block)
+        cuuint64_t dims[4] = {(cuuint64_t)g.c_in, (cuuint64_t)g.w_out, (cuuint64_t)g.h_out, (cuuint64_t)g.n};
+        cuuint64_t strides[3] = {(cuuint64_t)g.c_in * es, (cuuint64_t)g.w_out * g.c_in * es, (cuuint64_t)g.h_out * g.w_out * g.c_in * es};
+        cuuint32_t box[4] = {32, (cuuint32_t)po.tw, (cuuint32_t)po.th, (cuuint32_t)po.ni};
+        cuuint32_t estr[4] = {1, 1, 1, 1};
+        CUresult r = encode(&cp->tm_in, dt, 4, const_cast<void*>(mid), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(tf32x3 input) failed: " + std::to_string((int)r)); }
+    }
+    {   // split weights [2][c_out][c_in] viewed as (C_in, C_out, part); box (32, bn, 1) lands as bn K-major rows
+        cuuint64_t dims[3] = {(cuuint64_t)g.c_in, (cuuint64_t)g.c_out, 2};
+        cuuint64_t strides[2] = {(cuuint64_t)g.c_in * es, (cuuint64_t)g.c_out * g.c_in * es};
+        cuuint32_t box[3] = {32, (cuuint32_t)po.bn, 1};
+        cuuint32_t estr[3] = {1, 1, 1};
+        CUresult r = encode(&cp->tm_w, dt, 3, cp->w_split, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(tf32x3 weights) failed: " + std::to_string((int)r)); }
+    }
+    memset(cp->tm_o, 0, sizeof(cp->tm_o));
+    {   // plain NHWC, or the four (dy, dx) views of the nearest x2 map
+        const int up = g.upsample ? 2 : 1;
+        const cuuint64_t P = (cuuint64_t)out_pitch;
+        const cuuint64_t W2 = (cuuint64_t)g.w_out * up, H2 = (cuuint64_t)g.h_out * up;
+        for (int d = 0; d < (g.upsample ? 4 : 1); ++d) {
+            char* base = reinterpret_cast<char*>(out) + ((size_t)(d >> 1) * W2 + (d & 1)) * P * es;
+            cuuint64_t dims[4] = {(cuuint64_t)g.c_out, (cuuint64_t)g.w_out, (cuuint64_t)g.h_out, (cuuint64_t)g.n};
+            cuuint64_t strides[3] = {up * P * es, up * W2 * P * es, H2 * W2 * P * es};
+            cuuint32_t box[4] = {32, (cuuint32_t)po.tw, (cuuint32_t)po.th, (cuuint32_t)po.ni};
+            cuuint32_t estr[4] = {1, 1, 1, 1};
+            CUresult r = encode(&cp->tm_o[d], dt, 4, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(tf32x3 output) failed: " + std::to_string((int)r)); }
+        }
+    }
+    cp->smem_bytes = (size_t)po.smem_bytes;
+    cp->grid = dim3((unsigned)(p.items < opts.n_sms ? p.items : opts.n_sms), 1, 1);
+    char buf[160];
+    snprintf(buf, sizeof(buf), "conv_tc_kernel<pw,tf32x3,bn%d,%s>[%dx%dx%d,n%d,st%d,%s%s]", po.bn, g.upsample ? "up" : "noup",
+             po.ni, po.th, po.tw, p.splits, p.stages, g.act == FD_ACT_RELU6 ? "relu6" : "relu", reduce ? ",+skip(red)" : "");
+    cp->name = buf;
+    *res = cp;
+    return FD_OK;
+}
+
 const char* conv_tc_name(ConvTcPlan* cp) { return cp->name.c_str(); }
 
 template <typename T, int BN, bool RELU6>
@@ -370,7 +624,39 @@ static int conv_launch_t(ConvTcPlan* cp, cudaStream_t st) {
     }
 }
 
+template <int BN, bool RELU6>
+static int pw_tf32x3_launch_inst(ConvTcPlan* cp, cudaStream_t st) {
+    auto kern = conv_tc_tf32x3_kernel<BN, RELU6>;
+    static PerDeviceOnce attr_set;
+    int dev = -1;
+    FD_CUDA_OK(cudaGetDevice(&dev));
+    if (attr_set.need(dev)) {
+        FD_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        attr_set.done(dev);
+    }
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = cp->grid; cfg.blockDim = dim3(CV_THREADS); cfg.dynamicSmemBytes = cp->smem_bytes; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = cp->opts.pdl ? 1 : 0;
+    FD_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, cp->tm_in, cp->tm_w, cp->tm_o[0], cp->tm_o[1], cp->tm_o[2], cp->tm_o[3], cp->p,
+                                  cp->reduce));
+    FD_CUDA_OK(cudaGetLastError());
+    return FD_OK;
+}
+
+static int pw_tf32x3_launch(ConvTcPlan* cp, cudaStream_t st) {
+    const bool r6 = cp->act == FD_ACT_RELU6;
+    switch (cp->po.bn) {
+        case 64: return r6 ? pw_tf32x3_launch_inst<64, true>(cp, st) : pw_tf32x3_launch_inst<64, false>(cp, st);
+        case 128: return r6 ? pw_tf32x3_launch_inst<128, true>(cp, st) : pw_tf32x3_launch_inst<128, false>(cp, st);
+        default: return fail(FD_ERR_UNSUPPORTED, "no conv_tc_tf32x3_kernel instance for this bn");
+    }
+}
+
 int conv_tc_launch(ConvTcPlan* cp, cudaStream_t st) {
+    if (cp->tf32x3) return pw_tf32x3_launch(cp, st);
     return cp->dtype == FD_F16 ? conv_launch_t<__half>(cp, st) : conv_launch_t<__nv_bfloat16>(cp, st);
 }
 

@@ -3,6 +3,11 @@
 Replaces the Python layer loop of reference models.py:706-732 and every PyTorch operator it
 launches (SURVEY.md section 2b).  The engine is created lazily on the first forward so that
 modules restored by ``torch.load`` without ``__init__`` (reference main.py:49-57) work.
+
+fp32 inputs follow PyTorch's fp32 matmul precision: under ``torch.set_float32_matmul_precision('high')`` or ``'medium'``
+the pointwise convs (1x1 convs are matmuls) run as split TF32 on the tensor cores (plan option ``tf32x3``, within
+3*2^-22 of each exact product); under the default ``'highest'`` they stay on the fp32 SIMT kernels.  An explicit
+``set_option('tf32x3', v)`` wins over the precision setting.
 """
 import torch
 
@@ -88,6 +93,10 @@ class SkipAddEngine:
                 p.close()                      # an option stored before any plan existed turned out to be invalid
                 raise
             self.plans[key] = p
+        if x.dtype == torch.float32 and 'tf32x3' not in self.options:
+            want = int(torch.get_float32_matmul_precision() != 'highest')
+            if p.get_option('tf32x3') != want:
+                p.set_option('tf32x3', want)       # the steps are rebuilt on the next forward
         return p
 
     def __call__(self, x):

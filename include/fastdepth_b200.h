@@ -130,6 +130,13 @@ int fd_plan_set_stage_weights(fd_plan* plan, int stage,
  *                each CTA computes the depthwise half of a quarter (half) of the K-blocks, broadcasts its operand tiles to
  *                the others through distributed shared memory and runs the MMAs of one output-channel split (chosen by
  *                the planner's cost model for the small-map, many-channel blocks)  [default 1]
+ *   "tf32x3"     1 = in an fp32 plan on path 1, the pointwise half of every DWPW stage runs on the tensor cores as split
+ *                TF32: each operand is split into a TF32 high part and a TF32 low part (round to nearest), and each
+ *                product is a_lo*b_hi + a_hi*b_lo + a_hi*b_hi in an fp32 accumulator, within 3*2^-22 of the exact
+ *                product (plain TF32: about 2^-11).  The depthwise half, stem and head keep their fp32 SIMT kernels;
+ *                "chain" and "cluster" do not apply.  16-bit plans and path 0 ignore it.  fd_stage_buffer(which = 1)
+ *                still returns the depthwise intermediate.  (fastdepth_b200.engine sets it from
+ *                torch.get_float32_matmul_precision())  [default 0]
  *   "wait_sleep_ns" > 0: latency-tolerant roles of the fused block kernel (the TMA producer waiting for a
  *                free stage) sleep this many ns between barrier
  *                probes instead of spinning (the spinning waiters do not
@@ -207,6 +214,12 @@ int fd_debug_conv_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_o
  * {01, 10}); out[16 + 5 q .. 20 + 5 q] = {tap0, ny, nx, dy0, dx0} of phase q = 2 ry + rx (its taps tap0 .. tap0 + ny nx - 1
  * of the repacked weights, input offsets dy0 .. dy0 + ny - 1 by dx0 .. dx0 + nx - 1); out[36 + 2 g .. 37 + 2 g] = the phases
  * of group g (-1 = none), in execution order.  cap must be at least 44. */
+/* Debug (host only, needs no GPU): the tile plan of the split-TF32 pointwise step ("tf32x3") of one fp32 DWPW stage on an
+ * h_out x w_out map (upsample: its output is stored through the four views of the 2x map).  out[0..13] as in
+ * fd_debug_conv_plan, with kblocks counting 32-channel blocks (one 128-byte row of fp32); out[14] = bytes of one operand
+ * stage (16 KB of A + 2 x bn x 128 B of B, the weights' high and low parts), out[15] = 0.  cap must be at least 16. */
+int fd_debug_pw_tf32x3_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms, int* out, int cap);
+
 int fd_debug_convt_plan(int kind, int ksize, int h_in, int w_in, int n, int c_in, int c_out, int n_sms, int* out, int cap);
 
 /* Per-image depth metrics on device (reference metrics.py:31-55 applied per image, as

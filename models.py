@@ -268,7 +268,9 @@ class MobileNet(nn.Module):
         A CUDA tensor through the depthwise NNConv decoder ("MobileNet-NNConv5(dw)", reference README.md:37) takes the same
         fused sm_90a path as MobileNetSkipAdd, just without skips.  A CUDA fp16 / bf16 tensor through the dense decoder
         ("MobileNet-NNConv5", README.md:36) takes the engine too, with the decoder convs on conv_tc_kernel; the dense
-        decoder in fp32 stays on stock PyTorch (cuDNN may use TF32 tensor cores there, the project's fp32 path is SIMT).
+        decoder in fp32 stays on stock PyTorch (cuDNN may use TF32 tensor cores there; the project's fp32 path is SIMT,
+        except that the pointwise convs of the depthwise decoder run as split TF32 on the tensor cores under
+        ``torch.set_float32_matmul_precision('high' | 'medium')``).
         The DeConv and UpConv decoders route the same way as the dense NNConv decoder."""
         fused_ok = (x.is_cuda and not self.training and x.dim() == 4 and x.shape[1] == 3 and
                     x.shape[2] % 32 == 0 and x.shape[3] % 32 == 0)     # what the fused plan covers; anything else: stock PyTorch
@@ -331,7 +333,9 @@ class MobileNetSkipAdd(nn.Module):
         """One C-ABI call (``fd_forward``) on the caller's current CUDA stream.
 
         x: [N,3,H,W] CUDA tensor, fp32/fp16/bf16 (must match the module's parameter dtype),
-        any strides; H, W multiples of 32.  Returns a fresh contiguous [N,1,H,W] tensor of
+        any strides; H, W multiples of 32.  In fp32 the pointwise convs follow ``torch.get_float32_matmul_precision()``:
+        'highest' (the default) keeps them on fp32 SIMT kernels, 'high' / 'medium' runs them as split TF32 (three TF32
+        products per term) on the tensor cores.  Returns a fresh contiguous [N,1,H,W] tensor of
         the same dtype/device (reference models.py:706-732 contract)."""
         engine = self.__dict__.get('_fd_engine')
         if engine is None:
