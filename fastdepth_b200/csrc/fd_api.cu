@@ -15,6 +15,8 @@ namespace fd {
 BlockPlanOut block_tc_debug_plan(int ksize, int stride, int h_out, int w_out, int n, int c_in, int c_out, int head);
 ConvPlanOut conv_tc_debug_plan(int kind, int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms);
 ConvPlanOut pw_tf32x3_debug_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms);
+ConvPlanOut conv_tc_tf32x3_debug_plan(int kind, int ksize, int h_out, int w_out, int n, int c_in, int c_out, int upsample,
+                                      int n_sms);
 
 // ---- error state -----------------------------------------------------------------------
 static thread_local std::string g_last_error;
@@ -73,6 +75,10 @@ void conv_tc_destroy(ConvTcPlan* cp);
 const char* conv_tc_name(ConvTcPlan* cp);
 // the split-TF32 pointwise step of an fp32 DWPW stage (fd_conv_tc.cu)
 bool pw_tf32x3_supported(const StageGeom& g);
+bool conv_tc_tf32x3_supported(const StageGeom& g, int kind);
+int conv_tc_tf32x3_prepare(int kind, const StageGeom& g, const void* in, const float* w, const float* scale_dev,
+                           const float* bias_dev, void* out, const TcLaunchOpts& opts, ConvTcPlan** res);
+size_t conv_tc_split_bytes(ConvTcPlan* cp);
 int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w, const float* scale_dev, const float* bias_dev,
                       void* out, int out_pitch, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res);
 
@@ -130,6 +136,7 @@ struct fd_plan {
     int opt_cluster = 1;
     int opt_tf32x3 = 0;
     size_t workspace_bytes = 0;
+    size_t steps_bytes = 0;              // device memory the built steps hold (tf32x3: the split weights), freed with them
     // fd_pipeline_*: host batches flow H2D -> forward -> D2H through kPipeSlots device slots on three streams
     struct PipeSlot { void* x = nullptr; void* y = nullptr; cudaEvent_t up = nullptr, done = nullptr, down = nullptr; bool busy = false; };
     PipeSlot pipe[3];
@@ -176,6 +183,7 @@ static int dev_alloc(fd_plan* p, void** ptr, size_t bytes) {
 static void invalidate(fd_plan* p) {
     p->steps_valid = false;
     p->steps.clear();
+    p->steps_bytes = 0;
     for (auto& g : p->graphs) cudaGraphExecDestroy(g.exec);
     p->graphs.clear();
     for (auto& s : p->stages) {
@@ -265,7 +273,17 @@ static int build_steps(fd_plan* p) {
             st.alg_bytes = (px_in * g.c_in + px_out * (g.upsample || is_phased(kind) ? 4.0 : 1.0) * g.c_out) * es +
                            kk * g.c_in * g.c_out * es + 2.0 * g.c_out * 4;
             const int dtype = p->dtype;
-            if (p->opt_path == 1 && conv_tc_supported(dtype, g, kind)) {
+            if (dtype == FD_F32 && p->opt_path == 1 && p->opt_tf32x3 && conv_tc_tf32x3_supported(g, kind)) {
+                // fp32 under tf32x3: the same implicit GEMM as split TF32 (conv_tc_tf32x3_kernel), three TF32 products per
+                // term; the weights are split once into their TF32 high and low parts, a buffer twice the fp32 weights
+                int rc = conv_tc_tf32x3_prepare(kind, g, in, static_cast<const float*>(s.pw_w), s.pw_scale, s.pw_bias, s.out, lopts,
+                                                &s.ctc);
+                if (rc != FD_OK) return rc;
+                p->steps_bytes += conv_tc_split_bytes(s.ctc);
+                st.name = conv_tc_name(s.ctc);
+                ConvTcPlan* ctc = s.ctc;
+                st.run = [ctc](cudaStream_t stream, const void*, void*) { return conv_tc_launch(ctc, stream); };
+            } else if (p->opt_path == 1 && conv_tc_supported(dtype, g, kind)) {
                 int rc = conv_tc_prepare(dtype, kind, g, in, s.pw_w, s.pw_scale, s.pw_bias, s.out, lopts, &s.ctc);
                 if (rc != FD_OK) return rc;
                 st.name = conv_tc_name(s.ctc);
@@ -409,6 +427,7 @@ static int build_steps(fd_plan* p) {
                     int rc = pw_tf32x3_prepare(a.g, a.mid, static_cast<const float*>(a.pw_w), a.pw_scale, a.pw_bias, out, opitch,
                                                add ? 1 : 0, lopts, &s.ctc);
                     if (rc != FD_OK) return rc;
+                    p->steps_bytes += conv_tc_split_bytes(s.ctc);
                     q.name = conv_tc_name(s.ctc);
                     ConvTcPlan* ctc = s.ctc;
                     const bool copy = add && !inplace;
@@ -869,7 +888,7 @@ int fd_plan_launches_per_forward(fd_plan* p, int* n_launches) {
 
 int fd_plan_workspace_bytes(fd_plan* p, size_t* bytes) {
     if (!p || !bytes) return fail(FD_ERR_INVALID, "NULL argument");
-    *bytes = p->workspace_bytes;
+    *bytes = p->workspace_bytes + p->steps_bytes;
     return FD_OK;
 }
 
@@ -977,6 +996,23 @@ int fd_debug_pw_tf32x3_plan(int h_out, int w_out, int n, int c_in, int c_out, in
     const int v[16] = {q.ok, q.ni, q.th, q.tw, q.bn, q.stages, q.m_tiles, q.n_splits, q.items, q.waves, q.kblocks, q.smem_bytes,
                        q.useful_permille, (int)(q.cost > 2e9 ? 2e9 : q.cost), q.ok ? conv_stage_bytes_tf32x3(q.bn) : 0, 0};
     for (int i = 0; i < 16; ++i) out[i] = v[i];
+    return FD_OK;
+}
+
+int fd_debug_conv_tf32x3_plan(int kind, int ksize, int h, int w, int n, int c_in, int c_out, int upsample, int n_sms, int* out,
+                              int cap) {
+    if (!out || cap < 44) return fail(FD_ERR_INVALID, "need an int[44] output");
+    if (kind != FD_STAGE_CONV && !is_phased(kind)) return fail(FD_ERR_INVALID, "kind must be FD_STAGE_CONV, FD_STAGE_DECONV or FD_STAGE_UPCONV");
+    const ConvPlanOut q = conv_tc_tf32x3_debug_plan(kind, ksize, h, w, n, c_in, c_out, upsample, n_sms);
+    const int v[16] = {q.ok, q.ni, q.th, q.tw, q.bn, q.stages, q.m_tiles, q.n_splits, q.items, q.waves, q.kblocks, q.smem_bytes,
+                       q.useful_permille, (int)(q.cost > 2e9 ? 2e9 : q.cost), q.ok ? conv_stage_bytes_tf32x3(q.bn) : 0, q.groups};
+    for (int i = 0; i < 16; ++i) out[i] = v[i];
+    for (int ph = 0; ph < 4; ++ph) {
+        const int e[5] = {q.ph[ph].tap0, q.ph[ph].ny, q.ph[ph].nx, q.ph[ph].dy0, q.ph[ph].dx0};
+        for (int j = 0; j < 5; ++j) out[16 + 5 * ph + j] = q.ok && ph < q.n_phases ? e[j] : 0;
+    }
+    for (int g = 0; g < 4; ++g)
+        for (int j = 0; j < 2; ++j) out[36 + 2 * g + j] = q.ok ? q.group_ph[g][j] : -1;
     return FD_OK;
 }
 

@@ -16,7 +16,7 @@
 // two diagonal pairs {00, 11} and {01, 10}.  Items are ordered group-major, heaviest group first, and the cost model takes the
 // makespan of the persistent grid's static round-robin assignment over the real per-item tap counts.
 //
-// The split-TF32 pointwise instance (tf32x3: an fp32 1x1 conv as three TF32 products per term, fd_conv_tc.cu) has an fp32
+// The split-TF32 instance (tf32x3: an fp32 1x1, k x k or phased conv as three TF32 products per term, fd_conv_tc.cu) has an fp32
 // operand format: one 128-byte row holds 32 fp32 channels, so a K-block is 32 channels, and a stage holds the A box (16 KB)
 // plus two B boxes, the weights' TF32 high and low parts (2 x bn x 128 B).  Its MMA time counts three TF32 products per MAC
 // at the dense TF32 rate (1024 MAC / clock / SM, half the 16-bit rate); the consumers read A with ordinary shared loads (to
@@ -80,7 +80,7 @@ struct ConvPlanIn {
     int force_tile;            // -1 = the cost model chooses, else an index into kConvTiles
     int kind;                  // kConvKind*; 0 = CONV
     int force_group;           // phases per item of a DECONV / UPCONV stage: 0 = the cost model chooses, 1 = one, 2 = pairs
-    int tf32x3;                // 1: the split-TF32 pointwise instance (fp32 operands, 1x1 CONV only)
+    int tf32x3;                // 1: the split-TF32 instance (fp32 operands; 1x1 or k in {3, 5} CONV, DECONV, UPCONV)
 };
 struct ConvPlanOut {
     int ok;
@@ -181,7 +181,7 @@ inline ConvPlanOut plan_conv(const ConvPlanIn& q) {
     const bool phased = q.kind == kConvKindDeconv || q.kind == kConvKindUpconv;
     if (q.force_group && (!phased || q.force_group > 2)) return best;
     if (phased && (q.ksize < 3 || q.ksize > 9 || !(q.ksize & 1))) return best;
-    if (q.tf32x3 && (phased || q.ksize != 1)) return best;
+    if (q.tf32x3 && !phased && q.ksize != 1 && q.ksize != 3 && q.ksize != 5) return best;
     if (q.ksize < 1 || q.h_out < 1 || q.w_out < 1 || q.n < 1 || q.c_in < 8 || q.c_out < 8) return best;
     const int bns[3] = {64, 128, 256};
     for (int t = 0; t < kConvNumTiles; ++t) {

@@ -19,16 +19,20 @@
 // consumers' K loop come from the phase's {tap0, ny, nx, dy0, dx0}, and phase 2 ry + rx is stored through output view
 // tm_o[2 ry + rx] (the same four strided views as the upsample).  A CONV stage is one phase, the k x k square.
 //
-// conv_tc_tf32x3_kernel is the fp32 pointwise (1x1) conv of a DWPW stage as split TF32 (plan option "tf32x3"): the same
-// item decode, persistent item loop, operand ring and output views, with fp32 operands.  A K-block is 32 fp32 channels (one
-// 128-byte row); a stage is the A box {32 ch, tw, th, ni} of the depthwise intermediate plus two B boxes {32 ch, bn rows}, the
-// weights' TF32 high and low parts (split once when the plan is built).  The consumers split A themselves: each thread loads
+// conv_tc_tf32x3_kernel is an fp32 conv as split TF32 (plan option "tf32x3"): the pointwise (1x1) conv of a DWPW stage, and
+// the CONV / DECONV / UPCONV stages of the dense decoders.  The same item decode, persistent item loop, phase / tap loop,
+// operand ring and output views, with fp32 operands.  A K-block is 32 fp32 channels (one 128-byte row); a stage is the A box
+// {32 ch, tw, th, ni} of the input at the tap's offset (the depthwise intermediate of a DWPW stage) plus two B boxes
+// {32 ch, 1 tap, bn rows}, the tap's TF32 high and low weight parts (split once into [2][c_out][k*k][c_in] when the plan is
+// built; a pointwise step is one phase with one tap).  The consumers split A themselves: each thread loads
 // its wgmma A fragment from the swizzled tile, rounds it to a_hi = rna(a), a_lo = rna(a - a_hi), and per k8 step issues
 // a_lo b_hi, a_hi b_lo, a_hi b_hi (small terms first) into one fp32 accumulator, A from registers.  The epilogue applies the
 // BN affine and act in fp32 and stores [128 px][32 ch] fp32 tiles; a skip add is a TMA reduce-add (.add.f32) of that tile
-// into the skip tensor (or a copy of it), so the stage output is skip + up rounded once.  It is a sibling kernel rather
-// than an instance of conv_tc_kernel: producer, K loop and epilogue all differ (two B boxes, A through registers, three
-// MMAs per step, fp32 stores or reduce-adds), and the 16-bit instances stay exactly as they were.
+// into the skip tensor (or a copy of it), so the stage output is skip + up rounded once; a phased stage stores phase q
+// through view q.  It is a sibling kernel rather than an instance of conv_tc_kernel: producer, K loop and epilogue all
+// differ (two B boxes, A through registers, three MMAs per step, fp32 stores or reduce-adds), and the 16-bit instances stay
+// exactly as they were.
+#include <cstdint>
 #include <cstdio>
 #include <cstring>
 #include <new>
@@ -226,7 +230,7 @@ conv_tc_tf32x3_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_co
     }
     if (warp == CV_WARP_TMA && lane == 0) {
         tma_prefetch_desc(&tm_in); tma_prefetch_desc(&tm_w); tma_prefetch_desc(&tm_o0);
-        if (p.upsample) { tma_prefetch_desc(&tm_o1); tma_prefetch_desc(&tm_o2); tma_prefetch_desc(&tm_o3); }
+        if (p.upsample || p.phased) { tma_prefetch_desc(&tm_o1); tma_prefetch_desc(&tm_o2); tma_prefetch_desc(&tm_o3); }
     }
     pdl_launch_dependents();
     pdl_wait_prior_grid();
@@ -234,17 +238,26 @@ conv_tc_tf32x3_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_co
 
     if (warp == CV_WARP_TMA) {
         // =========================== TMA producer ===========================
+        // per phase of the item's group, per tap (ky, kx) and 32-channel K-block: the A box at the tap's offset (the OOB zero
+        // fill is the padding and the channel tail) and the tap's two B boxes; a pointwise step is one phase with one tap
         if (lane == 0) {
             Ring r;
             for (int w = blockIdx.x; w < p.items; w += gridDim.x) {
                 const ConvCoord c = conv_decode(p, w, BN);
-                for (int kb = 0; kb < p.kblocks; ++kb, r.next((uint32_t)p.stages)) {
-                    const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes, bar = smem_u32(&bars->full[r.s]);
-                    mbar_wait(smem_u32(&bars->empty[r.s]), r.ph ^ 1u);
-                    mbar_expect_tx(bar, (uint32_t)p.stage_bytes);
-                    tma_load_4d(st, &tm_in, bar, kb * 32, c.ox0, c.oy0, c.img0);
-                    tma_load_3d(st + CV_A_BYTES, &tm_w, bar, kb * 32, c.n0, 0);                  // high part
-                    tma_load_3d(st + CV_A_BYTES + BN * 128, &tm_w, bar, kb * 32, c.n0, 1);       // low part
+                for (int code = c.code; code != 0xF; code >>= 4) {
+                    const ConvPhase f = p.ph[code & 0xF];
+                    for (int ky = 0; ky < f.ny; ++ky)
+                        for (int kx = 0; kx < f.nx; ++kx) {
+                            const int tap = f.tap0 + ky * f.nx + kx;
+                            for (int kb = 0; kb < p.kblocks; ++kb, r.next((uint32_t)p.stages)) {
+                                const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes, bar = smem_u32(&bars->full[r.s]);
+                                mbar_wait(smem_u32(&bars->empty[r.s]), r.ph ^ 1u);
+                                mbar_expect_tx(bar, (uint32_t)p.stage_bytes);
+                                tma_load_4d(st, &tm_in, bar, kb * 32, c.ox0 + f.dx0 + kx, c.oy0 + f.dy0 + ky, c.img0);
+                                tma_load_4d(st + CV_A_BYTES, &tm_w, bar, kb * 32, tap, c.n0, 0);             // high part
+                                tma_load_4d(st + CV_A_BYTES + BN * 128, &tm_w, bar, kb * 32, tap, c.n0, 1);  // low part
+                            }
+                        }
                 }
             }
         }
@@ -260,73 +273,78 @@ conv_tc_tf32x3_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_co
         uint32_t stg_flip = 0;
         for (int w = blockIdx.x; w < p.items; w += gridDim.x) {
             const ConvCoord c = conv_decode(p, w, BN);
-            float acc[BN / 2];
+            for (int code = c.code; code != 0xF; code >>= 4) {           // the phases of this item's group, one after the other
+                const int q = code & 0xF;
+                const int ksteps = p.ph[q].ny * p.ph[q].nx * p.kblocks;
+                float acc[BN / 2];
 #pragma unroll
-            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-            for (int k = 0; k < p.kblocks; ++k) {
-                mbar_wait(smem_u32(&bars->full[r.s]), r.ph);
-                const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes;
-                const uint8_t* a_tile = smem + r.s * (uint32_t)p.stage_bytes;
-                // this thread's A fragments of the four k8 steps: channel 8 k4 + t (+ 4) of rows r0 and r0 + 8, split
-                uint32_t a_hi[4][4], a_lo[4][4];
+                for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+                for (int k = 0; k < ksteps; ++k) {
+                    mbar_wait(smem_u32(&bars->full[r.s]), r.ph);
+                    const uint32_t st = smem_base + r.s * (uint32_t)p.stage_bytes;
+                    const uint8_t* a_tile = smem + r.s * (uint32_t)p.stage_bytes;
+                    // this thread's A fragments of the four k8 steps: channel 8 k4 + t (+ 4) of rows r0 and r0 + 8, split
+                    uint32_t a_hi[4][4], a_lo[4][4];
 #pragma unroll
-                for (int k4 = 0; k4 < 4; ++k4)
+                    for (int k4 = 0; k4 < 4; ++k4)
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const int row = r0 + (e & 1) * 8, ch = 8 * k4 + t + (e >> 1) * 4;
-                        const float v = *reinterpret_cast<const float*>(a_tile + row * 128 + ((((uint32_t)ch >> 2) ^ sw) << 4) + (ch & 3) * 4);
-                        a_hi[k4][e] = rna_tf32(v);
-                        a_lo[k4][e] = rna_tf32(v - __uint_as_float(a_hi[k4][e]));
+                        for (int e = 0; e < 4; ++e) {
+                            const int row = r0 + (e & 1) * 8, ch = 8 * k4 + t + (e >> 1) * 4;
+                            const float v = *reinterpret_cast<const float*>(a_tile + row * 128 + ((((uint32_t)ch >> 2) ^ sw) << 4) + (ch & 3) * 4);
+                            a_hi[k4][e] = rna_tf32(v);
+                            a_lo[k4][e] = rna_tf32(v - __uint_as_float(a_hi[k4][e]));
+                        }
+                    const uint32_t bh = sw128_desc_lo(st + CV_A_BYTES), bl = sw128_desc_lo(st + CV_A_BYTES + BN * 128);
+                    wgmma_fence();
+#pragma unroll
+                    for (int k4 = 0; k4 < 4; ++k4) {               // +32 B (8 fp32 channels) per k8 step inside the 128-byte row
+                        wgmma_tf32_bn<BN>(acc, a_lo[k4], sw128_desc(bh + 2u * k4), (k > 0 || k4 > 0) ? 1u : 0u);
+                        wgmma_tf32_bn<BN>(acc, a_hi[k4], sw128_desc(bl + 2u * k4), 1u);
+                        wgmma_tf32_bn<BN>(acc, a_hi[k4], sw128_desc(bh + 2u * k4), 1u);
                     }
-                const uint32_t bh = sw128_desc_lo(st + CV_A_BYTES), bl = sw128_desc_lo(st + CV_A_BYTES + BN * 128);
-                wgmma_fence();
-#pragma unroll
-                for (int k4 = 0; k4 < 4; ++k4) {               // +32 B (8 fp32 channels) per k8 step inside the 128-byte row
-                    wgmma_tf32_bn<BN>(acc, a_lo[k4], sw128_desc(bh + 2u * k4), (k > 0 || k4 > 0) ? 1u : 0u);
-                    wgmma_tf32_bn<BN>(acc, a_hi[k4], sw128_desc(bl + 2u * k4), 1u);
-                    wgmma_tf32_bn<BN>(acc, a_hi[k4], sw128_desc(bh + 2u * k4), 1u);
+                    wgmma_commit();
+                    // the A registers are rewritten by the next step: wait for this step's MMAs, then release the stage
+                    wgmma_wait0();
+                    if (releaser) mbar_arrive(smem_u32(&bars->empty[r.s]));
+                    r.next((uint32_t)p.stages);
                 }
-                wgmma_commit();
-                // the A registers are rewritten by the next step: wait for this step's MMAs, then release the stage
-                wgmma_wait0();
-                if (releaser) mbar_arrive(smem_u32(&bars->empty[r.s]));
-                r.next((uint32_t)p.stages);
-            }
 
-            // per block of 32 output channels: registers -> BN affine + act (fp32) -> staging tile [128 px][32 ch] fp32
-            // (16-byte chunks XOR-swizzled like a SWIZZLE_128B box) -> TMA tensor stores or reduce-adds
+                // per block of 32 output channels: registers -> BN affine + act (fp32) -> staging tile [128 px][32 ch] fp32
+                // (16-byte chunks XOR-swizzled like a SWIZZLE_128B box) -> TMA tensor stores or reduce-adds
 #pragma unroll
-            for (int cb = 0; cb < BN / 32; ++cb) {
-                if (c.n0 + cb * 32 >= p.c_out) break;
-                uint8_t* stg = smem + stg_off + (stg_flip & 1u) * (uint32_t)kConvStg;
-                ++stg_flip;
-                const float2* aff = p.affine + c.n0 + cb * 32;
+                for (int cb = 0; cb < BN / 32; ++cb) {
+                    if (c.n0 + cb * 32 >= p.c_out) break;
+                    uint8_t* stg = smem + stg_off + (stg_flip & 1u) * (uint32_t)kConvStg;
+                    ++stg_flip;
+                    const float2* aff = p.affine + c.n0 + cb * 32;
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {                  // 8-column group i of this block
-                    const float4 af = __ldg(reinterpret_cast<const float4*>(aff + i * 8 + cq));     // (s0, s1, b0, b1)
-                    const int j = cb * 4 + i, cl = i * 8 + cq;
+                    for (int i = 0; i < 4; ++i) {                  // 8-column group i of this block
+                        const float4 af = __ldg(reinterpret_cast<const float4*>(aff + i * 8 + cq));     // (s0, s1, b0, b1)
+                        const int j = cb * 4 + i, cl = i * 8 + cq;
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int rr = r0 + 8 * h;
-                        float v0 = fmaxf(fmaf(acc[4 * j + 2 * h], af.x, af.z), 0.0f);
-                        float v1 = fmaxf(fmaf(acc[4 * j + 2 * h + 1], af.y, af.w), 0.0f);
-                        if (RELU6) { v0 = fminf(v0, 6.0f); v1 = fminf(v1, 6.0f); }
-                        *reinterpret_cast<float2*>(stg + rr * 128 + ((((uint32_t)cl >> 2) ^ sw) << 4) + (cl & 3) * 4) = make_float2(v0, v1);
+                        for (int h = 0; h < 2; ++h) {
+                            const int rr = r0 + 8 * h;
+                            float v0 = fmaxf(fmaf(acc[4 * j + 2 * h], af.x, af.z), 0.0f);
+                            float v1 = fmaxf(fmaf(acc[4 * j + 2 * h + 1], af.y, af.w), 0.0f);
+                            if (RELU6) { v0 = fminf(v0, 6.0f); v1 = fminf(v1, 6.0f); }
+                            *reinterpret_cast<float2*>(stg + rr * 128 + ((((uint32_t)cl >> 2) ^ sw) << 4) + (cl & 3) * 4) = make_float2(v0, v1);
+                        }
                     }
-                }
-                fence_proxy_async();
-                if (elected) bulk_wait_read0();
-                asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");
-                if (elected) {
-                    const uint32_t src = smem_u32(stg);
-                    const int cc = c.n0 + cb * 32;
-                    const int nv = p.upsample ? 4 : 1;
-                    for (int v = 0; v < nv; ++v) {
-                        const CUtensorMap* m = v == 0 ? &tm_o0 : v == 1 ? &tm_o1 : v == 2 ? &tm_o2 : &tm_o3;
-                        if (reduce) tma_reduce_add_4d(m, src, cc, c.ox0, c.oy0, c.img0);
-                        else tma_store_4d(m, src, cc, c.ox0, c.oy0, c.img0);
+                    fence_proxy_async();
+                    if (elected) bulk_wait_read0();
+                    asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(bar_n) : "memory");
+                    if (elected) {
+                        const uint32_t src = smem_u32(stg);
+                        const int cc = c.n0 + cb * 32;
+                        // phased: phase q through view q; else view 0, or all four views of the nearest x2 map
+                        const int v0 = p.phased ? q : 0, v1 = p.phased ? q + 1 : (p.upsample ? 4 : 1);
+                        for (int v = v0; v < v1; ++v) {
+                            const CUtensorMap* m = v == 0 ? &tm_o0 : v == 1 ? &tm_o1 : v == 2 ? &tm_o2 : &tm_o3;
+                            if (reduce) tma_reduce_add_4d(m, src, cc, c.ox0, c.oy0, c.img0);
+                            else tma_store_4d(m, src, cc, c.ox0, c.oy0, c.img0);
+                        }
+                        bulk_commit_group();
                     }
-                    bulk_commit_group();
                 }
             }
         }
@@ -346,7 +364,8 @@ struct ConvTcPlan {
     int dtype, act;
     TcLaunchOpts opts;
     float2* affine = nullptr;
-    float* w_split = nullptr;            // tf32x3: [2][c_out][c_in] fp32, the weights' TF32 high then low parts
+    float* w_split = nullptr;            // tf32x3: [2][c_out][k*k][c_in] fp32, the weights' TF32 high then low parts
+    size_t w_split_bytes = 0;
     int tf32x3 = 0, reduce = 0;
     std::string name;
 };
@@ -495,6 +514,15 @@ bool pw_tf32x3_supported(const StageGeom& g) {
     return g.c_in % 8 == 0 && g.c_out % 8 == 0 && get_tensor_map_encoder() != nullptr;
 }
 
+// the dense stages the split-TF32 step runs: CONV k in {3, 5} stride 1, DECONV k in {3, 5, 7, 9}, UPCONV k = 5
+bool conv_tc_tf32x3_supported(const StageGeom& g, int kind) {
+    if (g.c_in % 8 || g.c_out % 8) return false;
+    if (kind == kConvKindConv && ((g.ksize != 3 && g.ksize != 5) || g.stride != 1)) return false;
+    if (kind == kConvKindDeconv && g.ksize != 3 && g.ksize != 5 && g.ksize != 7 && g.ksize != 9) return false;
+    if (kind == kConvKindUpconv && g.ksize != 5) return false;
+    return get_tensor_map_encoder() != nullptr;
+}
+
 ConvPlanOut pw_tf32x3_debug_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms) {
     ConvPlanIn q{};
     q.ksize = 1; q.h_out = h_out; q.w_out = w_out; q.n = n; q.c_in = c_in; q.c_out = c_out; q.upsample = upsample;
@@ -502,21 +530,35 @@ ConvPlanOut pw_tf32x3_debug_plan(int h_out, int w_out, int n, int c_in, int c_ou
     return plan_conv(q);
 }
 
-// The split-TF32 pointwise step of an fp32 DWPW stage: `mid` is the stage's depthwise intermediate (NHWC fp32, c_in dense),
-// `w` its fp32 pointwise weights [c_out][c_in], `out` / `out_pitch` what the tiles are written to (g.upsample: through the
-// four views of the 2x map).  reduce = 1: the tiles are reduce-added into `out`, which already holds the skip tensor.
-// FD_CONV_TILE / FD_CONV_BN pin the planner's choice as for conv_tc_prepare.
-int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w, const float* scale_dev, const float* bias_dev,
-                      void* out, int out_pitch, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res) {
+ConvPlanOut conv_tc_tf32x3_debug_plan(int kind, int ksize, int h_out, int w_out, int n, int c_in, int c_out, int upsample,
+                                      int n_sms) {
+    ConvPlanIn q{};
+    q.ksize = ksize; q.h_out = h_out; q.w_out = w_out; q.n = n; q.c_in = c_in; q.c_out = c_out; q.upsample = upsample;
+    q.n_sms = n_sms; q.force_tile = -1; q.kind = kind; q.tf32x3 = 1;
+    return plan_conv(q);
+}
+
+// One split-TF32 step.  kind / ksize: a 1x1 CONV (the pointwise half of a DWPW stage), a k x k CONV, or a DECONV / UPCONV
+// as four phase convs at the input resolution.  `in` is NHWC fp32 of in_w x in_h pixels with in_pitch elements per pixel;
+// `w` the fp32 weights [c_out][k*k][c_in] (phase-major taps), split here once into [2][c_out][k*k][c_in] (TF32 high, then
+// low part); `out` / `out_pitch` what the tiles are written to (g.upsample: the four views of the 2x map; phased: phase q
+// through view q).  reduce = 1: the tiles are reduce-added into `out`, which already holds the skip tensor.
+// FD_CONV_TILE / FD_CONV_BN / FD_CONV_PHASE_GROUP pin the planner's choice as for conv_tc_prepare.
+static int tf32x3_prepare(int kind, int ksize, const StageGeom& g, const void* in, int in_w, int in_h, int in_pitch,
+                          const float* w, const float* scale_dev, const float* bias_dev, void* out, int out_pitch, int reduce,
+                          const TcLaunchOpts& opts, ConvTcPlan** res) {
     PFN_encodeTiled encode = get_tensor_map_encoder();
     if (!encode) return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    const bool phased = kind != kConvKindConv;
+    const bool pw = ksize == 1;
     ConvPlanIn q{};
-    q.ksize = 1; q.h_out = g.h_out; q.w_out = g.w_out; q.n = g.n; q.c_in = g.c_in; q.c_out = g.c_out; q.upsample = g.upsample;
-    q.n_sms = opts.n_sms; q.force_tile = -1; q.kind = kConvKindConv; q.tf32x3 = 1;
+    q.ksize = ksize; q.h_out = g.h_out; q.w_out = g.w_out; q.n = g.n; q.c_in = g.c_in; q.c_out = g.c_out; q.upsample = g.upsample;
+    q.n_sms = opts.n_sms; q.force_tile = -1; q.kind = kind; q.tf32x3 = 1;
     { const char* e = getenv("FD_CONV_TILE"); if (e && *e) q.force_tile = atoi(e); }
     { const char* e = getenv("FD_CONV_BN"); if (e && *e) q.force_bn = atoi(e); }
+    { const char* e = getenv("FD_CONV_PHASE_GROUP"); if (phased && e && *e) q.force_group = atoi(e); }
     const ConvPlanOut po = plan_conv(q);
-    if (!po.ok) return fail(FD_ERR_UNSUPPORTED, "tf32x3 pointwise step: no tile plan fits shared memory");
+    if (!po.ok) return fail(FD_ERR_UNSUPPORTED, "tf32x3 conv step: no tile plan fits shared memory");
     ConvTcPlan* cp = new (std::nothrow) ConvTcPlan();
     if (!cp) return fail(FD_ERR_CUDA, "out of host memory");
     cp->dtype = FD_F32; cp->act = g.act; cp->opts = opts; cp->po = po; cp->tf32x3 = 1; cp->reduce = reduce;
@@ -528,48 +570,55 @@ int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w, const
     p.splits = po.n_splits; p.items = po.items;
     p.kblocks = po.kblocks;
     p.stages = po.stages; p.stage_bytes = conv_stage_bytes_tf32x3(po.bn);
-    p.upsample = g.upsample;
+    p.upsample = g.upsample; p.phased = phased ? 1 : 0;
     memcpy(p.ph, po.ph, sizeof(p.ph));
-    for (int i = 0; i < 4; ++i) p.group_code[i] = 0xF;
-    p.group_code[0] = 0xF0;                        // one group: phase 0, the 1x1 "square"
+    for (int i = 0; i < 4; ++i) {
+        p.group_code[i] = 0xF;
+        for (int j = 1; j >= 0; --j)
+            if (po.group_ph[i][j] >= 0) p.group_code[i] = (p.group_code[i] << 4) | po.group_ph[i][j];
+    }
     auto magic = [](int d) { return (unsigned long long)((1ULL << 40) / (unsigned long long)d) + 1ULL; };
     p.mg_splits = magic(p.splits); p.mg_tx = magic(p.tiles_x); p.mg_ty = magic(p.tiles_y); p.mg_img = magic(p.img_tiles);
     const int n_pad = p.splits * po.bn;
-    const int wcount = g.c_in * g.c_out;
+    const int taps = ksize * ksize;
+    const size_t wcount = (size_t)g.c_out * taps * g.c_in;
+    if (wcount > (size_t)INT32_MAX / 2) { conv_tc_destroy(cp); return fail(FD_ERR_UNSUPPORTED, "tf32x3 conv step: weights too large"); }
+    cp->w_split_bytes = 2 * wcount * sizeof(float);
     if (cudaMalloc(&cp->affine, (size_t)n_pad * sizeof(float2)) != cudaSuccess ||
-        cudaMalloc(&cp->w_split, (size_t)2 * wcount * sizeof(float)) != cudaSuccess) {
+        cudaMalloc(&cp->w_split, cp->w_split_bytes) != cudaSuccess) {
         conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cudaMalloc failed"); }
     pack_conv_affine_kernel<<<(n_pad + 127) / 128, 128>>>(scale_dev, bias_dev, cp->affine, g.c_out, n_pad);
-    split_tf32_kernel<<<(wcount + 255) / 256, 256>>>(w, cp->w_split, wcount);
+    split_tf32_kernel<<<(unsigned)((wcount + 255) / 256), 256>>>(w, cp->w_split, (int)wcount);
     if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "tf32x3 weight packing failed"); }
     p.affine = cp->affine;
 
     const size_t es = 4;
     const CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-    {   // depthwise intermediate: NHWC (C, W, H, N), box (32, tw, th, ni); OOB -> 0 (the channel tail of the last K-block)
-        cuuint64_t dims[4] = {(cuuint64_t)g.c_in, (cuuint64_t)g.w_out, (cuuint64_t)g.h_out, (cuuint64_t)g.n};
-        cuuint64_t strides[3] = {(cuuint64_t)g.c_in * es, (cuuint64_t)g.w_out * g.c_in * es, (cuuint64_t)g.h_out * g.w_out * g.c_in * es};
+    {   // input: NHWC (C, W, H, N), box (32, tw, th, ni); OOB -> 0 (the conv's zero padding and the channel tail of the last K-block)
+        cuuint64_t dims[4] = {(cuuint64_t)g.c_in, (cuuint64_t)in_w, (cuuint64_t)in_h, (cuuint64_t)g.n};
+        cuuint64_t strides[3] = {(cuuint64_t)in_pitch * es, (cuuint64_t)in_w * in_pitch * es, (cuuint64_t)in_h * in_w * in_pitch * es};
         cuuint32_t box[4] = {32, (cuuint32_t)po.tw, (cuuint32_t)po.th, (cuuint32_t)po.ni};
         cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = encode(&cp->tm_in, dt, 4, const_cast<void*>(mid), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+        CUresult r = encode(&cp->tm_in, dt, 4, const_cast<void*>(in), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(tf32x3 input) failed: " + std::to_string((int)r)); }
     }
-    {   // split weights [2][c_out][c_in] viewed as (C_in, C_out, part); box (32, bn, 1) lands as bn K-major rows
-        cuuint64_t dims[3] = {(cuuint64_t)g.c_in, (cuuint64_t)g.c_out, 2};
-        cuuint64_t strides[2] = {(cuuint64_t)g.c_in * es, (cuuint64_t)g.c_out * g.c_in * es};
-        cuuint32_t box[3] = {32, (cuuint32_t)po.bn, 1};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = encode(&cp->tm_w, dt, 3, cp->w_split, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    {   // split weights [2][c_out][k*k][c_in] viewed as (C_in, taps, C_out, part); box (32, 1, bn, 1) lands as bn K-major rows
+        cuuint64_t dims[4] = {(cuuint64_t)g.c_in, (cuuint64_t)taps, (cuuint64_t)g.c_out, 2};
+        cuuint64_t strides[3] = {(cuuint64_t)g.c_in * es, (cuuint64_t)taps * g.c_in * es, (cuuint64_t)wcount * es};
+        cuuint32_t box[4] = {32, 1, (cuuint32_t)po.bn, 1};
+        cuuint32_t estr[4] = {1, 1, 1, 1};
+        CUresult r = encode(&cp->tm_w, dt, 4, cp->w_split, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(tf32x3 weights) failed: " + std::to_string((int)r)); }
     }
     memset(cp->tm_o, 0, sizeof(cp->tm_o));
-    {   // plain NHWC, or the four (dy, dx) views of the nearest x2 map
-        const int up = g.upsample ? 2 : 1;
+    {   // plain NHWC, or the four (dy, dx) views of the 2x map (nearest upsample, or the phases of a DECONV / UPCONV)
+        const bool views4 = g.upsample || phased;
+        const int up = views4 ? 2 : 1;
         const cuuint64_t P = (cuuint64_t)out_pitch;
         const cuuint64_t W2 = (cuuint64_t)g.w_out * up, H2 = (cuuint64_t)g.h_out * up;
-        for (int d = 0; d < (g.upsample ? 4 : 1); ++d) {
+        for (int d = 0; d < (views4 ? 4 : 1); ++d) {
             char* base = reinterpret_cast<char*>(out) + ((size_t)(d >> 1) * W2 + (d & 1)) * P * es;
             cuuint64_t dims[4] = {(cuuint64_t)g.c_out, (cuuint64_t)g.w_out, (cuuint64_t)g.h_out, (cuuint64_t)g.n};
             cuuint64_t strides[3] = {up * P * es, up * W2 * P * es, H2 * W2 * P * es};
@@ -583,12 +632,39 @@ int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w, const
     cp->smem_bytes = (size_t)po.smem_bytes;
     cp->grid = dim3((unsigned)(p.items < opts.n_sms ? p.items : opts.n_sms), 1, 1);
     char buf[160];
-    snprintf(buf, sizeof(buf), "conv_tc_kernel<pw,tf32x3,bn%d,%s>[%dx%dx%d,n%d,st%d,%s%s]", po.bn, g.upsample ? "up" : "noup",
-             po.ni, po.th, po.tw, p.splits, p.stages, g.act == FD_ACT_RELU6 ? "relu6" : "relu", reduce ? ",+skip(red)" : "");
+    const char* act = g.act == FD_ACT_RELU6 ? "relu6" : "relu";
+    if (pw)
+        snprintf(buf, sizeof(buf), "conv_tc_kernel<pw,tf32x3,bn%d,%s>[%dx%dx%d,n%d,st%d,%s%s]", po.bn, g.upsample ? "up" : "noup",
+                 po.ni, po.th, po.tw, p.splits, p.stages, act, reduce ? ",+skip(red)" : "");
+    else if (!phased)
+        snprintf(buf, sizeof(buf), "conv_tc_kernel<k%d,tf32x3,bn%d,%s>[%dx%dx%d,n%d,st%d,%s]", ksize, po.bn,
+                 g.upsample ? "up" : "noup", po.ni, po.th, po.tw, p.splits, p.stages, act);
+    else
+        snprintf(buf, sizeof(buf), "conv_tc_kernel<%s%d,tf32x3,bn%d,%s>[%dx%dx%d,n%d,st%d,%s]",
+                 kind == kConvKindDeconv ? "deconv" : "upconv", ksize, po.bn, po.groups == 2 ? "4ph2" : "4ph", po.ni, po.th, po.tw,
+                 p.splits, p.stages, act);
     cp->name = buf;
     *res = cp;
     return FD_OK;
 }
+
+// The split-TF32 pointwise step of an fp32 DWPW stage: `mid` is the stage's depthwise intermediate (NHWC fp32, c_in dense),
+// `w` its fp32 pointwise weights [c_out][c_in].
+int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w, const float* scale_dev, const float* bias_dev,
+                      void* out, int out_pitch, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res) {
+    return tf32x3_prepare(kConvKindConv, 1, g, mid, g.w_out, g.h_out, g.c_in, w, scale_dev, bias_dev, out, out_pitch, reduce,
+                          opts, res);
+}
+
+// The split-TF32 step of a dense fp32 CONV / DECONV / UPCONV stage (arguments as for conv_tc_prepare; `w` is the repacked
+// fp32 [c_out][k*k][c_in]).
+int conv_tc_tf32x3_prepare(int kind, const StageGeom& g, const void* in, const float* w, const float* scale_dev,
+                           const float* bias_dev, void* out, const TcLaunchOpts& opts, ConvTcPlan** res) {
+    return tf32x3_prepare(kind, g.ksize, g, in, g.w_in, g.h_in, g.in_pitch > 0 ? g.in_pitch : g.c_in, w, scale_dev, bias_dev, out,
+                          g.out_pitch > 0 ? g.out_pitch : g.c_out, 0, opts, res);
+}
+
+size_t conv_tc_split_bytes(ConvTcPlan* cp) { return cp->w_split_bytes; }
 
 const char* conv_tc_name(ConvTcPlan* cp) { return cp->name.c_str(); }
 
@@ -625,7 +701,7 @@ static int conv_launch_t(ConvTcPlan* cp, cudaStream_t st) {
 }
 
 template <int BN, bool RELU6>
-static int pw_tf32x3_launch_inst(ConvTcPlan* cp, cudaStream_t st) {
+static int tf32x3_launch_inst(ConvTcPlan* cp, cudaStream_t st) {
     auto kern = conv_tc_tf32x3_kernel<BN, RELU6>;
     static PerDeviceOnce attr_set;
     int dev = -1;
@@ -646,17 +722,17 @@ static int pw_tf32x3_launch_inst(ConvTcPlan* cp, cudaStream_t st) {
     return FD_OK;
 }
 
-static int pw_tf32x3_launch(ConvTcPlan* cp, cudaStream_t st) {
+static int tf32x3_launch(ConvTcPlan* cp, cudaStream_t st) {
     const bool r6 = cp->act == FD_ACT_RELU6;
     switch (cp->po.bn) {
-        case 64: return r6 ? pw_tf32x3_launch_inst<64, true>(cp, st) : pw_tf32x3_launch_inst<64, false>(cp, st);
-        case 128: return r6 ? pw_tf32x3_launch_inst<128, true>(cp, st) : pw_tf32x3_launch_inst<128, false>(cp, st);
+        case 64: return r6 ? tf32x3_launch_inst<64, true>(cp, st) : tf32x3_launch_inst<64, false>(cp, st);
+        case 128: return r6 ? tf32x3_launch_inst<128, true>(cp, st) : tf32x3_launch_inst<128, false>(cp, st);
         default: return fail(FD_ERR_UNSUPPORTED, "no conv_tc_tf32x3_kernel instance for this bn");
     }
 }
 
 int conv_tc_launch(ConvTcPlan* cp, cudaStream_t st) {
-    if (cp->tf32x3) return pw_tf32x3_launch(cp, st);
+    if (cp->tf32x3) return tf32x3_launch(cp, st);
     return cp->dtype == FD_F16 ? conv_launch_t<__half>(cp, st) : conv_launch_t<__nv_bfloat16>(cp, st);
 }
 

@@ -5,9 +5,11 @@ launches (SURVEY.md section 2b).  The engine is created lazily on the first forw
 modules restored by ``torch.load`` without ``__init__`` (reference main.py:49-57) work.
 
 fp32 inputs follow PyTorch's fp32 matmul precision: under ``torch.set_float32_matmul_precision('high')`` or ``'medium'``
-the pointwise convs (1x1 convs are matmuls) run as split TF32 on the tensor cores (plan option ``tf32x3``, within
-3*2^-22 of each exact product); under the default ``'highest'`` they stay on the fp32 SIMT kernels.  An explicit
-``set_option('tf32x3', v)`` wins over the precision setting.
+the pointwise convs (1x1 convs are matmuls) and the convs of the dense decoders (NNConv5 / NNConv3, DeConv<k>, UpConv:
+implicit GEMMs) run as split TF32 on the tensor cores (plan option ``tf32x3``, within 3*2^-22 of each exact product);
+under the default ``'highest'`` they stay on the fp32 SIMT kernels.  An explicit ``set_option('tf32x3', v)`` wins over the
+precision setting.  ``models.MobileNet`` hands an fp32 input with a dense decoder to the engine only under ``'high'`` or
+``'medium'``: split TF32 stays within the fp32 bound of 1e-3 where cuDNN's plain TF32 convs do not.
 """
 import torch
 

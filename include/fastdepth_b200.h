@@ -171,7 +171,9 @@ int fd_stage_buffer(fd_plan* plan, int stage, int which, void** dev_ptr,
                     int* n, int* h, int* w, int* c, int* c_stride);
 
 /* Bookkeeping used by bench.py.  A "step" is one kernel launch of fd_forward under the current
- * options (a DWPW stage is one fused step on path 1, a dw + a pw step on path 0). */
+ * options (a DWPW stage is one fused step on path 1, a dw + a pw step on path 0).  The workspace bytes include, once the
+ * steps are built, the device memory they hold: with "tf32x3", the split weights [2][c_out][k*k][c_in] fp32 of every
+ * split-TF32 step. */
 int fd_plan_launches_per_forward(fd_plan* plan, int* n_launches);
 int fd_plan_workspace_bytes(fd_plan* plan, size_t* bytes);
 int fd_plan_step_count(fd_plan* plan, int* n_steps);
@@ -221,6 +223,15 @@ int fd_debug_conv_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_o
 int fd_debug_pw_tf32x3_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms, int* out, int cap);
 
 int fd_debug_convt_plan(int kind, int ksize, int h_in, int w_in, int n, int c_in, int c_out, int n_sms, int* out, int cap);
+
+/* Debug (host only, needs no GPU): the tile plan of the split-TF32 step ("tf32x3") of one dense fp32 stage: kind
+ * FD_STAGE_CONV (ksize 1, 3 or 5; h x w = the conv resolution, upsample: the output goes through the four views of the 2x
+ * map), FD_STAGE_DECONV (ksize 3, 5, 7 or 9) or FD_STAGE_UPCONV (ksize 5) on an h x w input map.  out[0..13] as in
+ * fd_debug_conv_plan, with kblocks counting 32-channel blocks per tap; out[14] = bytes of one operand stage (16 KB of A +
+ * 2 x bn x 128 B of B), out[15] = the number of phase groups (items = m_tiles * n_splits * groups); out[16..43] the phase
+ * table and groups as in fd_debug_convt_plan (a CONV stage: phase 0 only).  cap must be at least 44. */
+int fd_debug_conv_tf32x3_plan(int kind, int ksize, int h, int w, int n, int c_in, int c_out, int upsample, int n_sms,
+                              int* out, int cap);
 
 /* Per-image depth metrics on device (reference metrics.py:31-55 applied per image, as
  * main.py:40-41,80-82 does at batch size 1).  pred: [n, hw] of `dtype`; target: [n, hw] fp32.
