@@ -76,11 +76,16 @@ const char* conv_tc_name(ConvTcPlan* cp);
 // the split-TF32 pointwise step of an fp32 DWPW stage (fd_conv_tc.cu)
 bool pw_tf32x3_supported(const StageGeom& g);
 bool conv_tc_tf32x3_supported(const StageGeom& g, int kind);
-int conv_tc_tf32x3_prepare(int kind, const StageGeom& g, const void* in, const float* w, const float* scale_dev,
+int conv_tc_tf32x3_prepare(int kind, const StageGeom& g, const void* in, const float* w_split, const float* scale_dev,
                            const float* bias_dev, void* out, const TcLaunchOpts& opts, ConvTcPlan** res);
-size_t conv_tc_split_bytes(ConvTcPlan* cp);
-int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w, const float* scale_dev, const float* bias_dev,
+int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w_split, const float* scale_dev, const float* bias_dev,
                       void* out, int out_pitch, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res);
+int tf32_split_weights(const float* w, size_t count, float* dst);
+// device memory a kernel plan holds: its packed / padded parameter copies
+size_t block_tc_param_bytes(BlockTcPlan* bp);
+size_t chain_tc_param_bytes(ChainTcPlan* cp);
+size_t stem_tc_param_bytes(StemTcPlan* sp);
+size_t conv_tc_param_bytes(ConvTcPlan* cp);
 
 static size_t dtype_size(int dtype) { return dtype == FD_F32 ? 4 : 2; }
 static bool is_phased(int kind) { return kind == FD_STAGE_DECONV || kind == FD_STAGE_UPCONV; }
@@ -91,7 +96,6 @@ struct Stage {
     StageGeom g{};
     int out_h = 0, out_w = 0;            // spatial size of the stage's output buffer (after upsample)
     void* out = nullptr;                 // NHWC [n,out_h,out_w,c_out]   (STEM/DWPW)
-    void* out_eff = nullptr;             // buffer the stage really writes (== a skip source when accumulating in place)
     void* out_alloc = nullptr;           // what this stage cudaMalloc'ed (out may be a channel slice of another stage's buffer)
     int out_c = 0;                       // channels the NEXT stage sees (c_out, or c_out + c_skip after a concat)
     int out_pitch = 0;                   // elements between pixels of `out`
@@ -104,14 +108,20 @@ struct Stage {
     float* pw_w_f32 = nullptr;           // stem: [27][c_out] tap-major ; head: [c_in]
     float* pw_scale = nullptr;
     float* pw_bias = nullptr;
+    float* w_split = nullptr;            // tf32x3: pw_w split into [2][...] fp32 TF32 high then low parts, shared by every step set
     float head_scale = 0.f, head_bias = 0.f;
     bool have_weights = false;
+};
+
+// What one step set built for one stage.
+struct StageRun {
     BlockTcPlan* tc = nullptr;
     StemTcPlan* stc = nullptr;
     ConvTcPlan* ctc = nullptr;
     ChainTcPlan* chain = nullptr;        // set on the FIRST stage of a run executed by the chain kernel
     int chained = 0;                     // 1: this stage runs inside a chain kernel (its own output buffer is only written if it is
                                          //    the run's last stage)
+    void* out_eff = nullptr;             // buffer the stage really writes (== a skip source when accumulating in place)
 };
 
 struct Step {
@@ -122,6 +132,16 @@ struct Step {
     std::function<int(cudaStream_t, const void*, void*)> run;
 };
 
+// The steps of a forward over images [0, n) of the plan's buffers.  Planner choices, grids, item counts and tensor maps
+// depend on n; the activation buffers, packed weights and split weights are the plan's and shared by every set.
+struct StepSet {
+    int n = 0;
+    std::vector<Step> steps;
+    std::vector<StageRun> runs;          // per stage
+    size_t bytes = 0;                    // device memory its kernel plans hold (packed parameter copies)
+    unsigned long long stamp = 0;
+};
+
 }  // namespace fd
 
 using namespace fd;
@@ -129,14 +149,14 @@ using namespace fd;
 struct fd_plan {
     int n = 0, h = 0, w = 0, dtype = 0, device = 0, n_sms = 132;
     std::vector<Stage> stages;
-    std::vector<Step> steps;
-    bool steps_valid = false;
+    std::vector<StepSet*> sets;          // built lazily per live batch size; LRU-bounded, the set of the plan's own n is kept
+    unsigned long long set_clock = 0;
     int opt_path = 1, opt_fold_head = 1, opt_graph = 1, opt_tma_epilogue = 1, opt_inplace_skip = 1, opt_pdl = 0, opt_wait_sleep_ns = 0;
     int opt_chain = 1;
     int opt_cluster = 1;
     int opt_tf32x3 = 0;
     size_t workspace_bytes = 0;
-    size_t steps_bytes = 0;              // device memory the built steps hold (tf32x3: the split weights), freed with them
+    size_t split_bytes = 0;              // device memory of the stages' split weights (tf32x3), freed with the step sets
     // fd_pipeline_*: host batches flow H2D -> forward -> D2H through kPipeSlots device slots on three streams
     struct PipeSlot { void* x = nullptr; void* y = nullptr; cudaEvent_t up = nullptr, done = nullptr, down = nullptr; bool busy = false; };
     PipeSlot pipe[3];
@@ -149,14 +169,15 @@ struct fd_plan {
     bool last_stream_set = false;
     void* l2_flush = nullptr;
     size_t l2_flush_bytes = 0;
-    // CUDA graph cache keyed on the (x, y) pointer pair: callers that rotate a few buffers (or let a
-    // caching allocator hand the same blocks back) replay; a new pair is captured once, LRU-evicted.
-    struct GraphEntry { const void* x; void* y; cudaGraphExec_t exec; unsigned long long stamp; };
+    // CUDA graph cache keyed on the (x, y) pointer pair and the batch size: callers that rotate a few buffers (or let a
+    // caching allocator hand the same blocks back) replay; a new key is captured once, LRU-evicted.
+    struct GraphEntry { const void* x; void* y; int n; cudaGraphExec_t exec; unsigned long long stamp; };
     std::vector<GraphEntry> graphs;
     unsigned long long graph_clock = 0;
     int graph_misses = 0;                // consecutive fd_forward calls that found no captured graph for their (x, y) pair
 };
 static const size_t kMaxGraphs = 8;
+static const size_t kMaxStepSets = 8;
 
 namespace fd {
 
@@ -180,19 +201,42 @@ static int dev_alloc(fd_plan* p, void** ptr, size_t bytes) {
     return FD_OK;
 }
 
+static void destroy_set(StepSet* ss) {
+    for (auto& r : ss->runs) {
+        if (r.tc) block_tc_destroy(r.tc);
+        if (r.stc) stem_tc_destroy(r.stc);
+        if (r.ctc) conv_tc_destroy(r.ctc);
+        if (r.chain) chain_tc_destroy(r.chain);
+    }
+    delete ss;
+}
+
+static StepSet* find_set(fd_plan* p, int n) {
+    for (StepSet* ss : p->sets)
+        if (ss->n == n) return ss;
+    return nullptr;
+}
+
+// weights or options changed: every step set, every graph and the split weights go
 static void invalidate(fd_plan* p) {
-    p->steps_valid = false;
-    p->steps.clear();
-    p->steps_bytes = 0;
     for (auto& g : p->graphs) cudaGraphExecDestroy(g.exec);
     p->graphs.clear();
-    for (auto& s : p->stages) {
-        if (s.tc) { block_tc_destroy(s.tc); s.tc = nullptr; }
-        if (s.stc) { stem_tc_destroy(s.stc); s.stc = nullptr; }
-        if (s.ctc) { conv_tc_destroy(s.ctc); s.ctc = nullptr; }
-        if (s.chain) { chain_tc_destroy(s.chain); s.chain = nullptr; }
-        s.chained = 0;
+    for (StepSet* ss : p->sets) destroy_set(ss);
+    p->sets.clear();
+    for (auto& s : p->stages) { cudaFree(s.w_split); s.w_split = nullptr; }
+    p->split_bytes = 0;
+}
+
+// the stage's pw_w ([c_out][k*k][c_in], fp32) split once into its TF32 high and low parts, for every step set
+static int split_weights(fd_plan* p, Stage& s, size_t count, const float** out) {
+    if (!s.w_split) {
+        FD_CUDA_OK(cudaMalloc(&s.w_split, 2 * count * sizeof(float)));
+        int rc = tf32_split_weights(static_cast<const float*>(s.pw_w), count, s.w_split);
+        if (rc != FD_OK) { cudaFree(s.w_split); s.w_split = nullptr; return rc; }
+        p->split_bytes += 2 * count * sizeof(float);
     }
+    *out = s.w_split;
+    return FD_OK;
 }
 
 // fp32 host array -> device array of the plan dtype (exact when the values came from that dtype)
@@ -211,12 +255,17 @@ static int upload_as_dtype(int dtype, const float* host, size_t count, void* dev
     return FD_OK;
 }
 
-static int build_steps(fd_plan* p) {
-    invalidate(p);
+// Build the steps of a forward over images [0, n) into `ss`: every stage's geometry with n images, over the plan's buffers.
+static int build_steps(fd_plan* p, int n, StepSet* ss) {
     const int ns = (int)p->stages.size();
     const double es = (double)dtype_size(p->dtype);
     for (auto& s : p->stages)
         if (!s.have_weights) return fail(FD_ERR_STATE, "fd_plan_set_stage_weights was not called for every stage");
+    ss->n = n;
+    ss->runs.assign(ns, StageRun());
+    std::vector<StageRun>& R = ss->runs;
+    std::vector<StageGeom> G(ns);
+    for (int i = 0; i < ns; ++i) { G[i] = p->stages[i].g; G[i].n = n; }
 
     TcLaunchOpts lopts;                   // every kernel plan keeps its own copy (no process-wide launch state)
     lopts.pdl = p->opt_pdl; lopts.sleep_ns = p->opt_wait_sleep_ns; lopts.n_sms = p->n_sms; lopts.cluster = p->opt_cluster;
@@ -230,38 +279,42 @@ static int build_steps(fd_plan* p) {
 
     for (int i = 0; i < ns; ++i) {
         Stage& s = p->stages[i];
-        const void* in = i > 0 ? p->stages[i - 1].out_eff : nullptr;
-        s.out_eff = s.out;
-        s.g.in_pitch = i > 0 ? p->stages[i - 1].out_pitch : 0;
-        s.g.out_pitch = s.out_pitch;
-        s.g.skip_pitch = (s.d.skip_src >= 0 && !s.d.skip_mode) ? p->stages[s.d.skip_src].out_pitch : s.out_pitch;
+        StageRun& r = R[i];
+        StageGeom& sg = G[i];
+        const void* in = i > 0 ? R[i - 1].out_eff : nullptr;
+        r.out_eff = s.out;
+        sg.in_pitch = i > 0 ? p->stages[i - 1].out_pitch : 0;
+        sg.out_pitch = s.out_pitch;
+        sg.skip_pitch = (s.d.skip_src >= 0 && !s.d.skip_mode) ? p->stages[s.d.skip_src].out_pitch : s.out_pitch;
         if (s.d.kind == FD_STAGE_STEM) {
             Step st;
             st.stage = i;
             st.name = "stem_kernel";
-            st.macs = (double)s.g.n * s.g.h_out * s.g.w_out * s.g.c_out * 27.0;
-            st.alg_bytes = ((double)s.g.n * 3 * s.g.h_in * s.g.w_in + (double)s.g.n * s.g.h_out * s.g.w_out * s.g.c_out) * es +
-                           29.0 * s.g.c_out * 4;
+            st.macs = (double)sg.n * sg.h_out * sg.w_out * sg.c_out * 27.0;
+            st.alg_bytes = ((double)sg.n * 3 * sg.h_in * sg.w_in + (double)sg.n * sg.h_out * sg.w_out * sg.c_out) * es +
+                           29.0 * sg.c_out * 4;
             Stage* sp = &s;
             const int dtype = p->dtype;
-            if (p->opt_path == 1 && stem_tc_supported(dtype, s.g)) {
-                int rc = stem_tc_prepare(dtype, s.g, s.pw_w_f32, s.pw_scale, s.pw_bias, s.out, lopts, &s.stc);
+            if (p->opt_path == 1 && stem_tc_supported(dtype, sg)) {
+                int rc = stem_tc_prepare(dtype, sg, s.pw_w_f32, s.pw_scale, s.pw_bias, s.out, lopts, &r.stc);
                 if (rc != FD_OK) return rc;
-                st.name = stem_tc_name(s.stc);
-                StemTcPlan* stc = s.stc;
+                ss->bytes += stem_tc_param_bytes(r.stc);
+                st.name = stem_tc_name(r.stc);
+                StemTcPlan* stc = r.stc;
                 st.run = [stc](cudaStream_t stream, const void* x, void*) { return stem_tc_launch(stc, x, stream); };
             } else {
-                st.run = [sp, dtype](cudaStream_t stream, const void* x, void*) {
-                    return launch_stem(dtype, x, sp->out, sp->pw_w_f32, sp->pw_scale, sp->pw_bias, sp->g, stream);
+                const StageGeom g = sg;
+                st.run = [sp, dtype, g](cudaStream_t stream, const void* x, void*) {
+                    return launch_stem(dtype, x, sp->out, sp->pw_w_f32, sp->pw_scale, sp->pw_bias, g, stream);
                 };
             }
-            p->steps.push_back(st);
+            ss->steps.push_back(st);
         } else if (is_conv(s.d.kind)) {
             // dense kxk conv: one implicit-GEMM step (path 1: conv_tc_kernel, else the SIMT conv_kernel); with the head folded
             // below the last upsample the stage stores at conv resolution and head_kernel<up2x> replicates.  DECONV / UPCONV:
             // the same step as four phase convs at the input resolution (g.h_out == g.h_in), k*k*c_in*c_out MACs per input
             // pixel, the 2h x 2w output written once (path 0: convt_kernel)
-            StageGeom g = s.g;
+            StageGeom g = sg;
             if (fold && &s == &last) g.upsample = 0;
             const int kind = s.d.kind;
             const double px_in = (double)g.n * g.h_in * g.w_in, px_out = (double)g.n * g.h_out * g.w_out;
@@ -276,18 +329,21 @@ static int build_steps(fd_plan* p) {
             if (dtype == FD_F32 && p->opt_path == 1 && p->opt_tf32x3 && conv_tc_tf32x3_supported(g, kind)) {
                 // fp32 under tf32x3: the same implicit GEMM as split TF32 (conv_tc_tf32x3_kernel), three TF32 products per
                 // term; the weights are split once into their TF32 high and low parts, a buffer twice the fp32 weights
-                int rc = conv_tc_tf32x3_prepare(kind, g, in, static_cast<const float*>(s.pw_w), s.pw_scale, s.pw_bias, s.out, lopts,
-                                                &s.ctc);
+                const float* w_split = nullptr;
+                int rc = split_weights(p, s, (size_t)g.c_out * g.ksize * g.ksize * g.c_in, &w_split);
                 if (rc != FD_OK) return rc;
-                p->steps_bytes += conv_tc_split_bytes(s.ctc);
-                st.name = conv_tc_name(s.ctc);
-                ConvTcPlan* ctc = s.ctc;
+                rc = conv_tc_tf32x3_prepare(kind, g, in, w_split, s.pw_scale, s.pw_bias, s.out, lopts, &r.ctc);
+                if (rc != FD_OK) return rc;
+                ss->bytes += conv_tc_param_bytes(r.ctc);
+                st.name = conv_tc_name(r.ctc);
+                ConvTcPlan* ctc = r.ctc;
                 st.run = [ctc](cudaStream_t stream, const void*, void*) { return conv_tc_launch(ctc, stream); };
             } else if (p->opt_path == 1 && conv_tc_supported(dtype, g, kind)) {
-                int rc = conv_tc_prepare(dtype, kind, g, in, s.pw_w, s.pw_scale, s.pw_bias, s.out, lopts, &s.ctc);
+                int rc = conv_tc_prepare(dtype, kind, g, in, s.pw_w, s.pw_scale, s.pw_bias, s.out, lopts, &r.ctc);
                 if (rc != FD_OK) return rc;
-                st.name = conv_tc_name(s.ctc);
-                ConvTcPlan* ctc = s.ctc;
+                ss->bytes += conv_tc_param_bytes(r.ctc);
+                st.name = conv_tc_name(r.ctc);
+                ConvTcPlan* ctc = r.ctc;
                 st.run = [ctc](cudaStream_t stream, const void*, void*) { return conv_tc_launch(ctc, stream); };
             } else if (kind == FD_STAGE_CONV) {
                 char nm[64];
@@ -306,8 +362,8 @@ static int build_steps(fd_plan* p) {
                     return launch_convt(dtype, kind, in, sp->pw_w, sp->out, sp->pw_scale, sp->pw_bias, g, stream);
                 };
             }
-            p->steps.push_back(st);
-        } else if (s.d.kind == FD_STAGE_DWPW && s.chained) {
+            ss->steps.push_back(st);
+        } else if (s.d.kind == FD_STAGE_DWPW && r.chained) {
             continue;                                 // executed by the chain kernel launched at the run's first stage
         } else if (s.d.kind == FD_STAGE_DWPW) {
             // ---- a run of 3x3 stride-1 blocks on a small map: ONE chain kernel (2-CTA clusters, activations stay in shared memory)
@@ -322,10 +378,10 @@ static int build_steps(fd_plan* p) {
                     bool is_skip_source = false;                              // ... and so must a tensor a decoder stage will add / concatenate
                     for (int k2 = j + 1; k2 < ns; ++k2) if (p->stages[k2].d.skip_src == j) is_skip_source = true;
                     BlockArgs b{};
-                    b.g = t.g;
+                    b.g = G[j];
                     b.g.in_pitch = j > 0 ? p->stages[j - 1].out_pitch : 0;
                     b.g.out_pitch = t.out_pitch;
-                    b.in = j > 0 ? p->stages[j - 1].out_eff : nullptr;
+                    b.in = j > 0 ? R[j - 1].out_eff : nullptr;
                     b.out = t.out;
                     b.dw_w = t.dw_w; b.dw_scale = t.dw_scale; b.dw_bias = t.dw_bias;
                     b.pw_w = t.pw_w; b.pw_scale = t.pw_scale; b.pw_bias = t.pw_bias;
@@ -335,8 +391,9 @@ static int build_steps(fd_plan* p) {
                 int len = (int)run.size();
                 while (len >= 2 && !chain_tc_supported(p->dtype, geoms.data(), len)) --len;
                 if (len >= 2) {
-                    int rc = chain_tc_prepare(p->dtype, run.data(), len, lopts, &s.chain);
+                    int rc = chain_tc_prepare(p->dtype, run.data(), len, lopts, &r.chain);
                     if (rc != FD_OK) return rc;
+                    ss->bytes += chain_tc_param_bytes(r.chain);
                     Step st;
                     st.stage = i + len - 1;                                   // reported under the run's last stage (the tensor it writes)
                     st.macs = 0; st.dw_macs = 0;
@@ -347,38 +404,38 @@ static int build_steps(fd_plan* p) {
                         st.dw_macs += px * g.c_in * 9.0;
                         st.macs += px * g.c_in * 9.0 + px * g.c_in * g.c_out;
                         wb += (double)g.c_in * 9 * 4 + 2.0 * g.c_in * 4 + (double)g.c_in * g.c_out * es + 2.0 * g.c_out * 4;
-                        p->stages[i + k2].chained = 1;
-                        p->stages[i + k2].out_eff = p->stages[i + k2].out;
+                        R[i + k2].chained = 1;
+                        R[i + k2].out_eff = p->stages[i + k2].out;
                     }
                     // algorithmic bytes of the MERGED stage (SURVEY.md 8d rule): external input once + external output once + weights once
                     st.alg_bytes = ((double)geoms[0].n * geoms[0].h_in * geoms[0].w_in * geoms[0].c_in +
                                     (double)geoms[len - 1].n * geoms[len - 1].h_out * geoms[len - 1].w_out * geoms[len - 1].c_out) * es + wb;
                     char nm[200];
-                    snprintf(nm, sizeof(nm), "%s{stages %d-%d}", chain_tc_name(s.chain), i, i + len - 1);
+                    snprintf(nm, sizeof(nm), "%s{stages %d-%d}", chain_tc_name(r.chain), i, i + len - 1);
                     st.name = nm;
-                    ChainTcPlan* cpn = s.chain;
+                    ChainTcPlan* cpn = r.chain;
                     st.run = [cpn](cudaStream_t stream, const void*, void*) { return chain_tc_launch(cpn, stream); };
-                    p->steps.push_back(st);
-                    s.chained = 1;
+                    ss->steps.push_back(st);
+                    r.chained = 1;
                     continue;
                 }
             }
             BlockArgs a{};
-            a.g = s.g;
+            a.g = sg;
             const bool folded_here = fold && (&s == &last);
             if (folded_here) a.g.upsample = 0;
             a.in = in;
             a.mid = s.mid;
             a.out = s.out;
-            a.skip = (s.d.skip_src >= 0 && !s.d.skip_mode) ? p->stages[s.d.skip_src].out_eff : nullptr;   // concat: the source wrote its slice itself
+            a.skip = (s.d.skip_src >= 0 && !s.d.skip_mode) ? R[s.d.skip_src].out_eff : nullptr;   // concat: the source wrote its slice itself
             a.dw_w = s.dw_w; a.dw_scale = s.dw_scale; a.dw_bias = s.dw_bias;
             a.pw_w = s.pw_w; a.pw_scale = s.pw_scale; a.pw_bias = s.pw_bias;
-            const double px_in = (double)s.g.n * s.g.h_in * s.g.w_in, px_out = (double)s.g.n * s.g.h_out * s.g.w_out;
+            const double px_in = (double)sg.n * sg.h_in * sg.w_in, px_out = (double)sg.n * sg.h_out * sg.w_out;
             const double up = a.g.upsample ? 4.0 : 1.0;
-            const double dw_macs = px_out * s.g.c_in * s.g.ksize * s.g.ksize, pw_macs = px_out * s.g.c_in * s.g.c_out;
-            const double w_bytes = (double)s.g.c_in * s.g.ksize * s.g.ksize * 4 + 2.0 * s.g.c_in * 4 +
-                                   (double)s.g.c_in * s.g.c_out * es + 2.0 * s.g.c_out * 4;
-            const double fused_bytes = (px_in * s.g.c_in + px_out * up * s.g.c_out * (a.skip ? 2.0 : 1.0)) * es + w_bytes;
+            const double dw_macs = px_out * sg.c_in * sg.ksize * sg.ksize, pw_macs = px_out * sg.c_in * sg.c_out;
+            const double w_bytes = (double)sg.c_in * sg.ksize * sg.ksize * 4 + 2.0 * sg.c_in * 4 +
+                                   (double)sg.c_in * sg.c_out * es + 2.0 * sg.c_out * 4;
+            const double fused_bytes = (px_in * sg.c_in + px_out * up * sg.c_out * (a.skip ? 2.0 : 1.0)) * es + w_bytes;
             const int dtype = p->dtype;
             const bool fuse_head = folded_here && p->opt_path == 1 && block_tc_supported(dtype, a.g, true);
             bool use_tc = p->opt_path == 1 && block_tc_supported(dtype, a.g, false);
@@ -386,35 +443,36 @@ static int build_steps(fd_plan* p) {
                 // decoder blocks with a skip accumulate INTO the skip tensor (TMA reduce-add): that buffer becomes the
                 // block's output and the skip never has to be read by the SM
                 const bool tma_epi = p->opt_tma_epilogue != 0;
-                if (tma_epi && p->opt_inplace_skip && a.skip != nullptr) { a.out = const_cast<void*>(a.skip); s.out_eff = a.out; }
-                int rc = fuse_head ? block_tc_prepare(dtype, a, head.pw_w_f32, head.head_scale, head.head_bias, head.g.act, nullptr, false, lopts, &s.tc)
-                                   : block_tc_prepare(dtype, a, nullptr, 0.f, 0.f, 0, nullptr, tma_epi && (a.skip == nullptr || a.skip == a.out), lopts, &s.tc);
+                if (tma_epi && p->opt_inplace_skip && a.skip != nullptr) { a.out = const_cast<void*>(a.skip); r.out_eff = a.out; }
+                int rc = fuse_head ? block_tc_prepare(dtype, a, head.pw_w_f32, head.head_scale, head.head_bias, head.g.act, nullptr, false, lopts, &r.tc)
+                                   : block_tc_prepare(dtype, a, nullptr, 0.f, 0.f, 0, nullptr, tma_epi && (a.skip == nullptr || a.skip == a.out), lopts, &r.tc);
                 if (rc != FD_OK) return rc;
+                ss->bytes += block_tc_param_bytes(r.tc);
                 Step st;
                 st.stage = i;
-                st.name = block_tc_name(s.tc);
-                st.macs = dw_macs + pw_macs + (fuse_head ? px_out * s.g.c_out : 0.0);
+                st.name = block_tc_name(r.tc);
+                st.macs = dw_macs + pw_macs + (fuse_head ? px_out * sg.c_out : 0.0);
                 st.dw_macs = dw_macs;
-                st.alg_bytes = fuse_head ? (px_in * s.g.c_in + px_out * 4.0) * es + w_bytes + s.g.c_out * 4.0 : fused_bytes;
-                BlockTcPlan* tc = s.tc;
+                st.alg_bytes = fuse_head ? (px_in * sg.c_in + px_out * 4.0) * es + w_bytes + sg.c_out * 4.0 : fused_bytes;
+                BlockTcPlan* tc = r.tc;
                 st.run = [tc](cudaStream_t stream, const void*, void* y) { return block_tc_launch(tc, stream, y); };
-                p->steps.push_back(st);
+                ss->steps.push_back(st);
                 head_fused = fuse_head;
             } else {
                 Step d;
                 d.stage = i;
-                d.name = s.g.ksize == 3 ? "dw_kernel<3>" : "dw_kernel<5>";
+                d.name = sg.ksize == 3 ? "dw_kernel<3>" : "dw_kernel<5>";
                 d.macs = dw_macs;
                 d.dw_macs = dw_macs;
-                d.alg_bytes = (px_in + px_out) * s.g.c_in * es + (double)s.g.c_in * (s.g.ksize * s.g.ksize + 2) * 4;
+                d.alg_bytes = (px_in + px_out) * sg.c_in * es + (double)sg.c_in * (sg.ksize * sg.ksize + 2) * 4;
                 d.run = [a, dtype](cudaStream_t stream, const void*, void*) { return launch_dw(dtype, a, stream); };
-                p->steps.push_back(d);
+                ss->steps.push_back(d);
                 Step q;
                 q.stage = i;
                 q.name = "pw_kernel";
                 q.macs = pw_macs;
-                q.alg_bytes = (px_out * s.g.c_in + px_out * up * s.g.c_out * (a.skip ? 2.0 : 1.0)) * es +
-                              (double)s.g.c_in * s.g.c_out * es + 2.0 * s.g.c_out * 4;
+                q.alg_bytes = (px_out * sg.c_in + px_out * up * sg.c_out * (a.skip ? 2.0 : 1.0)) * es +
+                              (double)sg.c_in * sg.c_out * es + 2.0 * sg.c_out * 4;
                 if (dtype == FD_F32 && p->opt_path == 1 && p->opt_tf32x3 && pw_tf32x3_supported(a.g)) {
                     // the pointwise half as split TF32 on wgmma (conv_tc_tf32x3_kernel).  A skip is added by a TMA reduce-add
                     // of the tiles: into the skip tensor itself (inplace_skip, which then becomes the stage output), or into
@@ -423,13 +481,15 @@ static int build_steps(fd_plan* p) {
                     const bool inplace = add && p->opt_inplace_skip;
                     void* out = inplace ? const_cast<void*>(a.skip) : a.out;
                     const int opitch = inplace ? a.g.skip_pitch : a.g.out_pitch;
-                    if (inplace) s.out_eff = out;
-                    int rc = pw_tf32x3_prepare(a.g, a.mid, static_cast<const float*>(a.pw_w), a.pw_scale, a.pw_bias, out, opitch,
-                                               add ? 1 : 0, lopts, &s.ctc);
+                    if (inplace) r.out_eff = out;
+                    const float* w_split = nullptr;
+                    int rc = split_weights(p, s, (size_t)a.g.c_out * a.g.c_in, &w_split);
                     if (rc != FD_OK) return rc;
-                    p->steps_bytes += conv_tc_split_bytes(s.ctc);
-                    q.name = conv_tc_name(s.ctc);
-                    ConvTcPlan* ctc = s.ctc;
+                    rc = pw_tf32x3_prepare(a.g, a.mid, w_split, a.pw_scale, a.pw_bias, out, opitch, add ? 1 : 0, lopts, &r.ctc);
+                    if (rc != FD_OK) return rc;
+                    ss->bytes += conv_tc_param_bytes(r.ctc);
+                    q.name = conv_tc_name(r.ctc);
+                    ConvTcPlan* ctc = r.ctc;
                     const bool copy = add && !inplace;
                     const void* skip = a.skip;
                     const size_t rows = (size_t)a.g.n * s.out_h * s.out_w, row_bytes = (size_t)a.g.c_out * 4;
@@ -442,33 +502,32 @@ static int build_steps(fd_plan* p) {
                 } else {
                     q.run = [a, dtype](cudaStream_t stream, const void*, void*) { return launch_pw(dtype, a, stream); };
                 }
-                p->steps.push_back(q);
+                ss->steps.push_back(q);
             }
         } else if (!head_fused) {  // HEAD (unless decode_conv6 already ran inside the last block's epilogue)
             const bool up = fold;
-            const int hh = up ? last.g.h_out : s.g.h_in, ww = up ? last.g.w_out : s.g.w_in;
-            const long long m_total = (long long)s.g.n * hh * ww;
+            const int hh = up ? last.g.h_out : sg.h_in, ww = up ? last.g.w_out : sg.w_in;
+            const long long m_total = (long long)sg.n * hh * ww;
             Step st;
             st.stage = i;
             st.name = up ? "head_kernel<up2x>" : "head_kernel";
-            st.macs = (double)m_total * s.g.c_in;
-            st.alg_bytes = ((double)m_total * s.g.c_in + (double)s.g.n * s.g.h_in * s.g.w_in) * es + s.g.c_in * 4.0;
+            st.macs = (double)m_total * sg.c_in;
+            st.alg_bytes = ((double)m_total * sg.c_in + (double)sg.n * sg.h_in * sg.w_in) * es + sg.c_in * 4.0;
             Stage* sp = &s;
             const int dtype = p->dtype;
-            const int c = s.g.c_in, act = s.g.act, ipitch = s.g.in_pitch;
+            const int c = sg.c_in, act = sg.act, ipitch = sg.in_pitch;
             st.run = [sp, in, dtype, m_total, c, ipitch, hh, ww, up, act](cudaStream_t stream, const void*, void* y) {
                 return launch_head(dtype, in, y, sp->pw_w_f32, sp->head_scale, sp->head_bias, m_total, c, ipitch, hh, ww, up ? 1 : 0,
                                    act, stream);
             };
-            p->steps.push_back(st);
+            ss->steps.push_back(st);
         }
     }
-    p->steps_valid = true;
     return FD_OK;
 }
 
-static int run_steps(fd_plan* p, const void* x, void* y, cudaStream_t st) {
-    for (auto& s : p->steps) {
+static int run_steps(const StepSet* ss, const void* x, void* y, cudaStream_t st) {
+    for (auto& s : ss->steps) {
         int rc = s.run(st, x, y);
         if (rc != FD_OK) return fail(rc, std::string(fd_last_error()) + " [stage " + std::to_string(s.stage) + ": " + s.name + "]");
     }
@@ -703,17 +762,48 @@ int fd_plan_get_option(fd_plan* p, const char* name, int* value) {
     return FD_OK;
 }
 
-static int ensure_steps(fd_plan* p) {
-    if (p->steps_valid) return FD_OK;
-    return build_steps(p);
+// The step set for batch size n, built on first use.  Beyond kMaxStepSets the least recently used set goes, with its graphs;
+// the set of the plan's own n stays (introspection describes it).
+static int ensure_steps(fd_plan* p, int n, StepSet** out) {
+    StepSet* ss = find_set(p, n);
+    if (!ss) {
+        if (p->sets.size() >= kMaxStepSets) {
+            size_t victim = p->sets.size();
+            for (size_t i = 0; i < p->sets.size(); ++i)
+                if (p->sets[i]->n != p->n && (victim == p->sets.size() || p->sets[i]->stamp < p->sets[victim]->stamp)) victim = i;
+            const int vn = p->sets[victim]->n;
+            for (size_t i = 0; i < p->graphs.size();)
+                if (p->graphs[i].n == vn) { cudaGraphExecDestroy(p->graphs[i].exec); p->graphs.erase(p->graphs.begin() + i); }
+                else ++i;
+            destroy_set(p->sets[victim]);
+            p->sets.erase(p->sets.begin() + victim);
+        }
+        ss = new StepSet();
+        int rc = build_steps(p, n, ss);
+        if (rc != FD_OK) { destroy_set(ss); return rc; }
+        p->sets.push_back(ss);
+    }
+    ss->stamp = ++p->set_clock;
+    *out = ss;
+    return FD_OK;
 }
 
-static int forward_enqueue(fd_plan* p, const void* x_dev, void* y_dev, cudaStream_t st);
+static int forward_enqueue(fd_plan* p, const StepSet* ss, const void* x_dev, void* y_dev, cudaStream_t st);
 
 int fd_forward(fd_plan* p, const void* x_dev, void* y_dev, void* stream) {
-    if (!p || !x_dev || !y_dev) return fail(FD_ERR_INVALID, "NULL argument");
+    if (!p) return fail(FD_ERR_INVALID, "NULL argument");
+    return fd_forward_batch(p, p->n, x_dev, y_dev, stream);
+}
+
+int fd_forward_batch(fd_plan* p, int n, const void* x_dev, void* y_dev, void* stream) {
+    if (!p) return fail(FD_ERR_INVALID, "NULL argument");
+    if (n < 1 || n > p->n)
+        return fail(FD_ERR_INVALID, "batch size " + std::to_string(n) + " is outside [1, " + std::to_string(p->n) +
+                                        "], the plan's batch capacity");
+    if (!x_dev || !y_dev) return fail(FD_ERR_INVALID, "NULL argument");
     DeviceGuard guard(p->device);
-    int rc = ensure_steps(p);
+    StepSet* ss = nullptr;
+    int rc = ensure_steps(p, n, &ss);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     // A plan owns ONE set of activation buffers: a forward enqueued on another stream than the previous one first waits for that
@@ -721,7 +811,7 @@ int fd_forward(fd_plan* p, const void* x_dev, void* y_dev, void* stream) {
     // is spelled with several plans (fastdepth_b200.engine.ForwardLanes).
     if (!p->last_done) FD_CUDA_OK(cudaEventCreateWithFlags(&p->last_done, cudaEventDisableTiming));
     if (p->last_stream_set && p->last_stream != st) FD_CUDA_OK(cudaStreamWaitEvent(st, p->last_done, 0));
-    rc = forward_enqueue(p, x_dev, y_dev, st);
+    rc = forward_enqueue(p, ss, x_dev, y_dev, st);
     if (rc) return rc;
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
     if (cudaStreamIsCapturing(st, &cs) == cudaSuccess && cs == cudaStreamCaptureStatusNone) {
@@ -731,13 +821,13 @@ int fd_forward(fd_plan* p, const void* x_dev, void* y_dev, void* stream) {
     return FD_OK;
 }
 
-static int forward_enqueue(fd_plan* p, const void* x_dev, void* y_dev, cudaStream_t st) {
+static int forward_enqueue(fd_plan* p, const StepSet* ss, const void* x_dev, void* y_dev, cudaStream_t st) {
     int rc = FD_OK;
-    if (!p->opt_graph) return run_steps(p, x_dev, y_dev, st);
+    if (!p->opt_graph) return run_steps(ss, x_dev, y_dev, st);
 
-    // Replay from a CUDA graph captured for this (x, y) pair.
+    // Replay from a CUDA graph captured for this (x, y, n).
     for (auto& g : p->graphs)
-        if (g.x == x_dev && g.y == y_dev) {
+        if (g.x == x_dev && g.y == y_dev && g.n == ss->n) {
             g.stamp = ++p->graph_clock;
             p->graph_misses = 0;
             FD_CUDA_OK(cudaGraphLaunch(g.exec, st));
@@ -748,7 +838,7 @@ static int forward_enqueue(fd_plan* p, const void* x_dev, void* y_dev, cudaStrea
     // pair repeats again (19 PDL-chained launches cost far less than one capture).
     if (++p->graph_misses > 2 * (int)kMaxGraphs) {
         if (p->graph_misses > (1 << 30)) p->graph_misses = 2 * (int)kMaxGraphs + 1;
-        return run_steps(p, x_dev, y_dev, st);
+        return run_steps(ss, x_dev, y_dev, st);
     }
     cudaStream_t cap;
     FD_CUDA_OK(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
@@ -756,7 +846,7 @@ static int forward_enqueue(fd_plan* p, const void* x_dev, void* y_dev, cudaStrea
     cudaGraphExec_t exec = nullptr;
     cudaError_t e = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
     if (e == cudaSuccess) {
-        rc = run_steps(p, x_dev, y_dev, cap);
+        rc = run_steps(ss, x_dev, y_dev, cap);
         e = cudaStreamEndCapture(cap, &graph);
         if (rc == FD_OK && e == cudaSuccess) e = cudaGraphInstantiate(&exec, graph, 0);
     }
@@ -771,7 +861,7 @@ static int forward_enqueue(fd_plan* p, const void* x_dev, void* y_dev, cudaStrea
         cudaGraphExecDestroy(p->graphs[victim].exec);
         p->graphs.erase(p->graphs.begin() + victim);
     }
-    p->graphs.push_back({x_dev, y_dev, exec, ++p->graph_clock});
+    p->graphs.push_back({x_dev, y_dev, ss->n, exec, ++p->graph_clock});
     FD_CUDA_OK(cudaGraphLaunch(exec, st));
     return FD_OK;
 }
@@ -855,10 +945,11 @@ int fd_pipeline_wait(fd_plan* p, unsigned long long ticket) {
 int fd_stage_buffer(fd_plan* p, int stage, int which, void** dev_ptr, int* n, int* h, int* w, int* c, int* c_stride) {
     if (!p || stage < 0 || stage >= (int)p->stages.size() || !dev_ptr) return fail(FD_ERR_INVALID, "bad argument");
     Stage& s = p->stages[stage];
+    const StepSet* full = find_set(p, p->n);
     int hh, ww, cc;
     void* ptr;
     if (which == 0) {
-        ptr = s.out_eff ? s.out_eff : s.out; hh = s.out_h; ww = s.out_w; cc = s.g.c_out;
+        ptr = full && full->runs[stage].out_eff ? full->runs[stage].out_eff : s.out; hh = s.out_h; ww = s.out_w; cc = s.g.c_out;
         // with decode_conv6 folded below the last upsample the last block writes its low-res output
         if (p->opt_fold_head && stage == (int)p->stages.size() - 2 && s.d.upsample && s.d.skip_src < 0) { hh = s.g.h_out; ww = s.g.w_out; }
     } else if (which == 1) {
@@ -880,15 +971,20 @@ int fd_stage_buffer(fd_plan* p, int stage, int which, void** dev_ptr, int* n, in
 int fd_plan_launches_per_forward(fd_plan* p, int* n_launches) {
     if (!p || !n_launches) return fail(FD_ERR_INVALID, "NULL argument");
     DeviceGuard guard(p->device);
-    int rc = ensure_steps(p);
+    StepSet* ss = nullptr;
+    int rc = ensure_steps(p, p->n, &ss);
     if (rc) return rc;
-    *n_launches = (int)p->steps.size();
+    *n_launches = (int)ss->steps.size();
     return FD_OK;
 }
 
 int fd_plan_workspace_bytes(fd_plan* p, size_t* bytes) {
     if (!p || !bytes) return fail(FD_ERR_INVALID, "NULL argument");
-    *bytes = p->workspace_bytes + p->steps_bytes;
+    // the packed parameter copies of the plan's own step set are not counted; every smaller batch's set adds its own
+    size_t sets = 0;
+    for (const StepSet* ss : p->sets)
+        if (ss->n != p->n) sets += ss->bytes;
+    *bytes = p->workspace_bytes + p->split_bytes + sets;
     return FD_OK;
 }
 
@@ -897,10 +993,11 @@ int fd_plan_step_count(fd_plan* p, int* n_steps) { return fd_plan_launches_per_f
 int fd_plan_step_info(fd_plan* p, int step, int* stage, double* alg_bytes, double* macs, char* kernel_name, int name_cap) {
     if (!p) return fail(FD_ERR_INVALID, "NULL plan");
     DeviceGuard guard(p->device);
-    int rc = ensure_steps(p);
+    StepSet* ss = nullptr;
+    int rc = ensure_steps(p, p->n, &ss);
     if (rc) return rc;
-    if (step < 0 || step >= (int)p->steps.size()) return fail(FD_ERR_INVALID, "bad step index");
-    const Step& s = p->steps[step];
+    if (step < 0 || step >= (int)ss->steps.size()) return fail(FD_ERR_INVALID, "bad step index");
+    const Step& s = ss->steps[step];
     if (stage) *stage = s.stage;
     if (alg_bytes) *alg_bytes = s.alg_bytes;
     if (macs) *macs = s.macs;
@@ -914,10 +1011,11 @@ int fd_plan_step_info(fd_plan* p, int step, int* stage, double* alg_bytes, doubl
 int fd_plan_step_macs(fd_plan* p, int step, double* dw_macs, double* dense_macs) {
     if (!p) return fail(FD_ERR_INVALID, "NULL plan");
     DeviceGuard guard(p->device);
-    int rc = ensure_steps(p);
+    StepSet* ss = nullptr;
+    int rc = ensure_steps(p, p->n, &ss);
     if (rc) return rc;
-    if (step < 0 || step >= (int)p->steps.size()) return fail(FD_ERR_INVALID, "bad step index");
-    const Step& s = p->steps[step];
+    if (step < 0 || step >= (int)ss->steps.size()) return fail(FD_ERR_INVALID, "bad step index");
+    const Step& s = ss->steps[step];
     if (dw_macs) *dw_macs = s.dw_macs;
     if (dense_macs) *dense_macs = s.macs - s.dw_macs;
     return FD_OK;
@@ -927,28 +1025,29 @@ int fd_plan_time_steps(fd_plan* p, const void* x_dev, void* y_dev, void* stream,
                        float* ms_out) {
     if (!p || !x_dev || !y_dev || !ms_out || iters <= 0) return fail(FD_ERR_INVALID, "bad argument");
     DeviceGuard guard(p->device);
-    int rc = ensure_steps(p);
+    StepSet* ss = nullptr;
+    int rc = ensure_steps(p, p->n, &ss);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (flush_l2 && !p->l2_flush) {
         p->l2_flush_bytes = size_t(256) << 20;               // > the 50 MB L2
         FD_CUDA_OK(cudaMalloc(&p->l2_flush, p->l2_flush_bytes));
     }
-    rc = run_steps(p, x_dev, y_dev, st);                      // make every intermediate valid
+    rc = run_steps(ss, x_dev, y_dev, st);                     // make every intermediate valid
     if (rc) return rc;
     cudaEvent_t e0, e1;
     FD_CUDA_OK(cudaEventCreate(&e0));
     FD_CUDA_OK(cudaEventCreate(&e1));
-    for (size_t i = 0; i < p->steps.size() && rc == FD_OK; ++i) {
-        for (int k = 0; k < warmup && rc == FD_OK; ++k) rc = p->steps[i].run(st, x_dev, y_dev);
+    for (size_t i = 0; i < ss->steps.size() && rc == FD_OK; ++i) {
+        for (int k = 0; k < warmup && rc == FD_OK; ++k) rc = ss->steps[i].run(st, x_dev, y_dev);
         float total = 0.f;
         for (int k = 0; k < iters && rc == FD_OK; ++k) {
             if (flush_l2) cudaMemsetAsync(p->l2_flush, k & 0xff, p->l2_flush_bytes, st);
             cudaEventRecord(e0, st);
-            rc = p->steps[i].run(st, x_dev, y_dev);
+            rc = ss->steps[i].run(st, x_dev, y_dev);
             cudaEventRecord(e1, st);
             cudaError_t e = cudaEventSynchronize(e1);
-            if (e != cudaSuccess) { rc = fail(FD_ERR_CUDA, std::string("step ") + p->steps[i].name + ": " + cudaGetErrorString(e)); break; }
+            if (e != cudaSuccess) { rc = fail(FD_ERR_CUDA, std::string("step ") + ss->steps[i].name + ": " + cudaGetErrorString(e)); break; }
             float ms = 0.f;
             cudaEventElapsedTime(&ms, e0, e1);
             total += ms;
@@ -963,13 +1062,15 @@ int fd_plan_time_steps(fd_plan* p, const void* x_dev, void* y_dev, void* stream,
 int fd_plan_trace_stage(fd_plan* p, int stage, void* y_dev, void* stream, unsigned long long* out_host, int cap, int* rows, int* cols) {
     if (!p || stage < 0 || stage >= (int)p->stages.size() || !out_host || !rows || !cols) return fail(FD_ERR_INVALID, "bad argument");
     DeviceGuard guard(p->device);
-    int rc = ensure_steps(p);
+    StepSet* ss = nullptr;
+    int rc = ensure_steps(p, p->n, &ss);
     if (rc) return rc;
     if (cap < 12 * 256) return fail(FD_ERR_INVALID, "trace buffer too small (need 3072 entries)");
     if (is_conv(p->stages[stage].d.kind)) return fail(FD_ERR_INVALID, "the stage timeline exists for fused block kernels only");
-    if (p->stages[stage].chain) return chain_tc_trace(p->stages[stage].chain, (cudaStream_t)stream, out_host, rows, cols);
-    if (!p->stages[stage].tc) return fail(FD_ERR_STATE, "stage does not run the fused block kernel");
-    return block_tc_trace(p->stages[stage].tc, (cudaStream_t)stream, y_dev, out_host, rows, cols);
+    const StageRun& r = ss->runs[stage];
+    if (r.chain) return chain_tc_trace(r.chain, (cudaStream_t)stream, out_host, rows, cols);
+    if (!r.tc) return fail(FD_ERR_STATE, "stage does not run the fused block kernel");
+    return block_tc_trace(r.tc, (cudaStream_t)stream, y_dev, out_host, rows, cols);
 }
 
 int fd_debug_block_plan(int ksize, int stride, int h_out, int w_out, int n, int c_in, int c_out, int head, int* out, int cap) {

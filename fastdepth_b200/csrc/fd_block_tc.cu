@@ -823,6 +823,9 @@ int block_tc_launch(BlockTcPlan* bp, cudaStream_t st, void* head_out) {
     return bp->dtype == FD_F16 ? launch_t<__half>(bp, st) : launch_t<__nv_bfloat16>(bp, st);
 }
 
+size_t block_tc_param_bytes(BlockTcPlan* bp) {
+    return (size_t)bp->p.kblocks * bp->p.dwp_bytes + (size_t)bp->p.cpad_all * (sizeof(float2) + sizeof(float));
+}
 const char* block_tc_name(BlockTcPlan* bp) { return bp->name.c_str(); }
 
 BlockPlanOut block_tc_debug_plan(int ksize, int stride, int h_out, int w_out, int n, int c_in, int c_out, int head) {

@@ -446,6 +446,7 @@ struct ChainTcPlan {
     int dtype, relu6;
     TcLaunchOpts opts;
     std::vector<void*> owned;
+    size_t owned_bytes = 0;
     std::string name;
 };
 
@@ -473,6 +474,7 @@ void chain_tc_destroy(ChainTcPlan* cp) {
     delete cp;
 }
 const char* chain_tc_name(ChainTcPlan* cp) { return cp->name.c_str(); }
+size_t chain_tc_param_bytes(ChainTcPlan* cp) { return cp->owned_bytes; }
 
 int chain_tc_prepare(int dtype, const BlockArgs* layers, int n_layers, const TcLaunchOpts& opts, ChainTcPlan** out) {
     PFN_encodeTiled encode = get_tensor_map_encoder();
@@ -520,6 +522,7 @@ int chain_tc_prepare(int dtype, const BlockArgs* layers, int n_layers, const TcL
             cudaFree(dwp); rc = fail(FD_ERR_CUDA, "cudaMalloc failed"); break;
         }
         cp->owned.push_back(dwp); cp->owned.push_back(aff);
+        cp->owned_bytes += (size_t)L.kblocks * CH_DWP + (size_t)L.n_pad * sizeof(float2);
         const int tot = L.kblocks * 64;
         if (dtype == FD_F16) chain_pack_dwp_kernel<__half><<<(tot + 127) / 128, 128>>>(layers[l].dw_w, layers[l].dw_scale, layers[l].dw_bias, (uint8_t*)dwp, g.c_in, L.kblocks);
         else chain_pack_dwp_kernel<__nv_bfloat16><<<(tot + 127) / 128, 128>>>(layers[l].dw_w, layers[l].dw_scale, layers[l].dw_bias, (uint8_t*)dwp, g.c_in, L.kblocks);

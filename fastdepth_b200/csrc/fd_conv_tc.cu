@@ -364,8 +364,7 @@ struct ConvTcPlan {
     int dtype, act;
     TcLaunchOpts opts;
     float2* affine = nullptr;
-    float* w_split = nullptr;            // tf32x3: [2][c_out][k*k][c_in] fp32, the weights' TF32 high then low parts
-    size_t w_split_bytes = 0;
+    size_t affine_bytes = 0;
     int tf32x3 = 0, reduce = 0;
     std::string name;
 };
@@ -402,7 +401,6 @@ bool conv_tc_supported(int dtype, const StageGeom& g, int kind) {
 void conv_tc_destroy(ConvTcPlan* cp) {
     if (!cp) return;
     cudaFree(cp->affine);
-    cudaFree(cp->w_split);
     delete cp;
 }
 
@@ -450,7 +448,8 @@ int conv_tc_prepare(int dtype, int kind, const StageGeom& g, const void* in, con
     auto magic = [](int d) { return (unsigned long long)((1ULL << 40) / (unsigned long long)d) + 1ULL; };
     p.mg_splits = magic(p.splits); p.mg_tx = magic(p.tiles_x); p.mg_ty = magic(p.tiles_y); p.mg_img = magic(p.img_tiles);
     const int n_pad = p.splits * po.bn;
-    if (cudaMalloc(&cp->affine, (size_t)n_pad * sizeof(float2)) != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cudaMalloc failed"); }
+    cp->affine_bytes = (size_t)n_pad * sizeof(float2);
+    if (cudaMalloc(&cp->affine, cp->affine_bytes) != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cudaMalloc failed"); }
     pack_conv_affine_kernel<<<(n_pad + 127) / 128, 128>>>(scale_dev, bias_dev, cp->affine, g.c_out, n_pad);
     if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "conv affine packing failed"); }
     p.affine = cp->affine;
@@ -540,13 +539,13 @@ ConvPlanOut conv_tc_tf32x3_debug_plan(int kind, int ksize, int h_out, int w_out,
 
 // One split-TF32 step.  kind / ksize: a 1x1 CONV (the pointwise half of a DWPW stage), a k x k CONV, or a DECONV / UPCONV
 // as four phase convs at the input resolution.  `in` is NHWC fp32 of in_w x in_h pixels with in_pitch elements per pixel;
-// `w` the fp32 weights [c_out][k*k][c_in] (phase-major taps), split here once into [2][c_out][k*k][c_in] (TF32 high, then
-// low part); `out` / `out_pitch` what the tiles are written to (g.upsample: the four views of the 2x map; phased: phase q
+// `w_split` the fp32 weights [c_out][k*k][c_in] (phase-major taps) split into [2][c_out][k*k][c_in] (TF32 high, then
+// low part, by tf32_split_weights; the caller owns it and may share it between steps); `out` / `out_pitch` what the tiles are written to (g.upsample: the four views of the 2x map; phased: phase q
 // through view q).  reduce = 1: the tiles are reduce-added into `out`, which already holds the skip tensor.
 // FD_CONV_TILE / FD_CONV_BN / FD_CONV_PHASE_GROUP pin the planner's choice as for conv_tc_prepare.
 static int tf32x3_prepare(int kind, int ksize, const StageGeom& g, const void* in, int in_w, int in_h, int in_pitch,
-                          const float* w, const float* scale_dev, const float* bias_dev, void* out, int out_pitch, int reduce,
-                          const TcLaunchOpts& opts, ConvTcPlan** res) {
+                          const float* w_split, const float* scale_dev, const float* bias_dev, void* out, int out_pitch,
+                          int reduce, const TcLaunchOpts& opts, ConvTcPlan** res) {
     PFN_encodeTiled encode = get_tensor_map_encoder();
     if (!encode) return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const bool phased = kind != kConvKindConv;
@@ -582,14 +581,10 @@ static int tf32x3_prepare(int kind, int ksize, const StageGeom& g, const void* i
     const int n_pad = p.splits * po.bn;
     const int taps = ksize * ksize;
     const size_t wcount = (size_t)g.c_out * taps * g.c_in;
-    if (wcount > (size_t)INT32_MAX / 2) { conv_tc_destroy(cp); return fail(FD_ERR_UNSUPPORTED, "tf32x3 conv step: weights too large"); }
-    cp->w_split_bytes = 2 * wcount * sizeof(float);
-    if (cudaMalloc(&cp->affine, (size_t)n_pad * sizeof(float2)) != cudaSuccess ||
-        cudaMalloc(&cp->w_split, cp->w_split_bytes) != cudaSuccess) {
-        conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cudaMalloc failed"); }
+    cp->affine_bytes = (size_t)n_pad * sizeof(float2);
+    if (cudaMalloc(&cp->affine, cp->affine_bytes) != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cudaMalloc failed"); }
     pack_conv_affine_kernel<<<(n_pad + 127) / 128, 128>>>(scale_dev, bias_dev, cp->affine, g.c_out, n_pad);
-    split_tf32_kernel<<<(unsigned)((wcount + 255) / 256), 256>>>(w, cp->w_split, (int)wcount);
-    if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "tf32x3 weight packing failed"); }
+    if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "tf32x3 affine packing failed"); }
     p.affine = cp->affine;
 
     const size_t es = 4;
@@ -608,7 +603,7 @@ static int tf32x3_prepare(int kind, int ksize, const StageGeom& g, const void* i
         cuuint64_t strides[3] = {(cuuint64_t)g.c_in * es, (cuuint64_t)taps * g.c_in * es, (cuuint64_t)wcount * es};
         cuuint32_t box[4] = {32, 1, (cuuint32_t)po.bn, 1};
         cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = encode(&cp->tm_w, dt, 4, cp->w_split, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+        CUresult r = encode(&cp->tm_w, dt, 4, const_cast<float*>(w_split), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { conv_tc_destroy(cp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(tf32x3 weights) failed: " + std::to_string((int)r)); }
     }
@@ -649,22 +644,30 @@ static int tf32x3_prepare(int kind, int ksize, const StageGeom& g, const void* i
 }
 
 // The split-TF32 pointwise step of an fp32 DWPW stage: `mid` is the stage's depthwise intermediate (NHWC fp32, c_in dense),
-// `w` its fp32 pointwise weights [c_out][c_in].
-int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w, const float* scale_dev, const float* bias_dev,
+// `w_split` its split pointwise weights [2][c_out][c_in].
+int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w_split, const float* scale_dev, const float* bias_dev,
                       void* out, int out_pitch, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res) {
-    return tf32x3_prepare(kConvKindConv, 1, g, mid, g.w_out, g.h_out, g.c_in, w, scale_dev, bias_dev, out, out_pitch, reduce,
+    return tf32x3_prepare(kConvKindConv, 1, g, mid, g.w_out, g.h_out, g.c_in, w_split, scale_dev, bias_dev, out, out_pitch, reduce,
                           opts, res);
 }
 
-// The split-TF32 step of a dense fp32 CONV / DECONV / UPCONV stage (arguments as for conv_tc_prepare; `w` is the repacked
-// fp32 [c_out][k*k][c_in]).
-int conv_tc_tf32x3_prepare(int kind, const StageGeom& g, const void* in, const float* w, const float* scale_dev,
+// The split-TF32 step of a dense fp32 CONV / DECONV / UPCONV stage (arguments as for conv_tc_prepare; `w_split` is the
+// repacked fp32 [c_out][k*k][c_in] split into [2][c_out][k*k][c_in]).
+int conv_tc_tf32x3_prepare(int kind, const StageGeom& g, const void* in, const float* w_split, const float* scale_dev,
                            const float* bias_dev, void* out, const TcLaunchOpts& opts, ConvTcPlan** res) {
-    return tf32x3_prepare(kind, g.ksize, g, in, g.w_in, g.h_in, g.in_pitch > 0 ? g.in_pitch : g.c_in, w, scale_dev, bias_dev, out,
+    return tf32x3_prepare(kind, g.ksize, g, in, g.w_in, g.h_in, g.in_pitch > 0 ? g.in_pitch : g.c_in, w_split, scale_dev, bias_dev, out,
                           g.out_pitch > 0 ? g.out_pitch : g.c_out, 0, opts, res);
 }
 
-size_t conv_tc_split_bytes(ConvTcPlan* cp) { return cp->w_split_bytes; }
+// Split `count` fp32 weights into dst[2][count]: the TF32 high parts, then the low parts.  Synchronous.
+int tf32_split_weights(const float* w, size_t count, float* dst) {
+    if (count > (size_t)INT32_MAX) return fail(FD_ERR_UNSUPPORTED, "tf32x3: weights too large");
+    split_tf32_kernel<<<(unsigned)((count + 255) / 256), 256>>>(w, dst, (int)count);
+    if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) return fail(FD_ERR_CUDA, "tf32x3 weight split failed");
+    return FD_OK;
+}
+
+size_t conv_tc_param_bytes(ConvTcPlan* cp) { return cp->affine_bytes; }
 
 const char* conv_tc_name(ConvTcPlan* cp) { return cp->name.c_str(); }
 

@@ -295,6 +295,7 @@ int stem_tc_prepare(int dtype, const StageGeom& g, const float* w27_dev, const f
     return FD_OK;
 }
 
+size_t stem_tc_param_bytes(StemTcPlan* sp) { return (size_t)sp->p.n_pad * (64 * 2 + sizeof(float2)); }
 const char* stem_tc_name(StemTcPlan* sp) { return sp->name.c_str(); }
 
 // x may change from call to call (the caller's tensor): re-encode the input tensor map when it does.  Under CUDA-graph

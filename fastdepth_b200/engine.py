@@ -10,6 +10,11 @@ implicit GEMMs) run as split TF32 on the tensor cores (plan option ``tf32x3``, w
 under the default ``'highest'`` they stay on the fp32 SIMT kernels.  An explicit ``set_option('tf32x3', v)`` wins over the
 precision setting.  ``models.MobileNet`` hands an fp32 input with a dense decoder to the engine only under ``'high'`` or
 ``'medium'``: split TF32 stays within the fp32 bound of 1e-3 where cuDNN's plain TF32 convs do not.
+
+One plan per (device, H, W, dtype) is live at a time.  A batch no larger than its capacity runs on it (the C-ABI builds
+the steps for that batch size once, over the plan's buffers and weights; ``fd_forward_batch``); a larger batch replaces it
+with a plan sized for that batch.  So an evaluation with a short last batch, or a serving loop that sees many batch sizes,
+holds one set of activation buffers and packed weights instead of one per batch size.
 """
 import torch
 
@@ -21,7 +26,7 @@ _SUPPORTED = (torch.float32, torch.float16, torch.bfloat16)
 class SkipAddEngine:
     def __init__(self, module):
         self.module = module
-        self.plans = {}          # (device index, n, h, w, dtype) -> Plan
+        self.plans = {}          # (device index, h, w, dtype) -> Plan (its n: the largest batch seen since the last refresh)
         self.signature = None
         self.options = {}
 
@@ -61,7 +66,9 @@ class SkipAddEngine:
             raise
 
     # -- forward ---------------------------------------------------------------------------------
-    def plan_for(self, x):
+    def plan_for(self, x, exact=False):
+        """The plan that runs ``x``: the live plan of its (device, H, W, dtype) if its capacity holds ``x.shape[0]`` images
+        (``exact``: equals it, as the host pipeline needs), else a new plan sized for ``x`` that replaces it."""
         m = self.module
         if m.training:
             raise RuntimeError("fastdepth_b200 is inference-only: call model.eval() first "
@@ -84,8 +91,11 @@ class SkipAddEngine:
         if sig != self.signature:
             self.refresh()
             self.signature = sig
-        key = (x.device.index, n, h, w, x.dtype)
+        key = (x.device.index, h, w, x.dtype)
         p = self.plans.get(key)
+        if p is not None and (n > p.n or (exact and n != p.n)):
+            del self.plans[key]       # freed with its last reference (a pending host-pipeline ticket holds one)
+            p = None
         if p is None:
             p = _plan.Plan.from_module(m, n, h, w, x.dtype, x.device.index)
             try:
@@ -173,7 +183,7 @@ class ForwardLanes:
         CUDA tensor of the batch's shape/dtype (selects the plan).  Returns a handle for ``wait``."""
         lane = self.next
         self.next = (self.next + 1) % len(self.engines)
-        p = self.engines[lane].plan_for(like)
+        p = self.engines[lane].plan_for(like, exact=True)      # the host pipeline moves the plan's full batch
         return lane, p, p.pipeline_submit(x_host, y_host)
 
     @staticmethod

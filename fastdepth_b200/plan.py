@@ -203,7 +203,8 @@ def _fp(a):
 
 
 class Plan:
-    """Owns one ``fd_plan`` (fixed N,H,W,dtype,device).  Thin: every method is one C-ABI call."""
+    """Owns one ``fd_plan`` (H,W,dtype,device and a batch capacity N; ``forward`` runs any batch up to N).  Thin: every
+    method is one C-ABI call."""
 
     def __init__(self, descs, weights, names, n, h, w, dtype, device_index):
         self.lib = _lib.load()
@@ -235,8 +236,14 @@ class Plan:
         _lib.check(self.lib.fd_plan_get_option(self.handle, name.encode(), ctypes.byref(v)))
         return v.value
 
-    def forward(self, x, y, stream_ptr):
-        _lib.check(self.lib.fd_forward(self.handle, x.data_ptr(), y.data_ptr(), stream_ptr))
+    def forward(self, x, y, stream_ptr, n=None):
+        """Forward of the first ``n`` images (default ``x.shape[0]``), 1 <= n <= the plan's n; a smaller batch runs on
+        the plan's buffers through ``fd_forward_batch``."""
+        n = x.shape[0] if n is None else int(n)
+        if n == self.n:
+            _lib.check(self.lib.fd_forward(self.handle, x.data_ptr(), y.data_ptr(), stream_ptr))
+        else:
+            _lib.check(self.lib.fd_forward_batch(self.handle, n, x.data_ptr(), y.data_ptr(), stream_ptr))
 
     def forward_host(self, x_host, y_host, stream_ptr):
         _lib.check(self.lib.fd_forward_host(self.handle, x_host.data_ptr(), y_host.data_ptr(), stream_ptr))

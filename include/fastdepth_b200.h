@@ -151,6 +151,14 @@ int fd_plan_get_option(fd_plan* plan, const char* name, int* value);
  * Replaces: pred = model(input)  (reference main.py:74-75 -> models.py:706-732). */
 int fd_forward(fd_plan* plan, const void* x_dev, void* y_dev, void* stream);
 
+/* The same forward over the first n images, 1 <= n <= the plan's N: x_dev is [n,3,H,W] and y_dev [n,1,H,W], and nothing
+ * is read or written past image n (FD_ERR_INVALID for any other n).  The result equals that of a plan built for n, bit for
+ * bit.  The plan builds the steps for n on first use (planner choices, grids, tensor maps) over its own activation buffers,
+ * packed weights and split weights; it keeps up to 8 such step sets, least recently used first out (the set of its own N is
+ * always kept), and captures graphs per (x_dev, y_dev, n).  fd_forward(plan, ...) is fd_forward_batch(plan, N, ...).
+ * fd_forward_host and fd_pipeline_* always run N images. */
+int fd_forward_batch(fd_plan* plan, int n, const void* x_dev, void* y_dev, void* stream);
+
 /* Same, end to end from HOST buffers: H2D copy of x, forward, D2H copy of y, then waits for
  * the stream.  (reference main.py:68 input.cuda() ... main.py:85-98 pred.cpu()) */
 int fd_forward_host(fd_plan* plan, const void* x_host, void* y_host, void* stream);
@@ -171,9 +179,11 @@ int fd_stage_buffer(fd_plan* plan, int stage, int which, void** dev_ptr,
                     int* n, int* h, int* w, int* c, int* c_stride);
 
 /* Bookkeeping used by bench.py.  A "step" is one kernel launch of fd_forward under the current
- * options (a DWPW stage is one fused step on path 1, a dw + a pw step on path 0).  The workspace bytes include, once the
+ * options (a DWPW stage is one fused step on path 1, a dw + a pw step on path 0); the step functions, fd_plan_time_steps,
+ * fd_plan_trace_stage and fd_stage_buffer describe the steps of the plan's own N.  The workspace bytes include, once the
  * steps are built, the device memory they hold: with "tf32x3", the split weights [2][c_out][k*k][c_in] fp32 of every
- * split-TF32 step. */
+ * split-TF32 step (once, shared by every batch size), and the packed parameter copies of every step set fd_forward_batch
+ * built for a batch size below N. */
 int fd_plan_launches_per_forward(fd_plan* plan, int* n_launches);
 int fd_plan_workspace_bytes(fd_plan* plan, size_t* bytes);
 int fd_plan_step_count(fd_plan* plan, int* n_steps);
