@@ -55,6 +55,7 @@ SIGNATURES = {
     'fd_debug_conv_plan': (ctypes.c_int, [ctypes.c_int] * 7 + [_c_int_p, ctypes.c_int]),
     'fd_debug_convt_plan': (ctypes.c_int, [ctypes.c_int] * 8 + [_c_int_p, ctypes.c_int]),
     'fd_debug_pw_tf32x3_plan': (ctypes.c_int, [ctypes.c_int] * 7 + [_c_int_p, ctypes.c_int]),
+    'fd_debug_pw_plan': (ctypes.c_int, [ctypes.c_int] * 7 + [_c_int_p, ctypes.c_int]),
     'fd_debug_conv_tf32x3_plan': (ctypes.c_int, [ctypes.c_int] * 9 + [_c_int_p, ctypes.c_int]),
     'fd_metrics_accumulate': (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp,
                                              ctypes.c_int, _vp]),

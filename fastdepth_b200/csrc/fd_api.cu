@@ -15,6 +15,7 @@ namespace fd {
 BlockPlanOut block_tc_debug_plan(int ksize, int stride, int h_out, int w_out, int n, int c_in, int c_out, int head);
 ConvPlanOut conv_tc_debug_plan(int kind, int ksize, int h_out, int w_out, int n, int c_in, int c_out, int n_sms);
 ConvPlanOut pw_tf32x3_debug_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms);
+ConvPlanOut pw_tc_debug_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms);
 ConvPlanOut conv_tc_tf32x3_debug_plan(int kind, int ksize, int h_out, int w_out, int n, int c_in, int c_out, int upsample,
                                       int n_sms);
 
@@ -81,6 +82,13 @@ int conv_tc_tf32x3_prepare(int kind, const StageGeom& g, const void* in, const f
 int pw_tf32x3_prepare(const StageGeom& g, const void* mid, const float* w_split, const float* scale_dev, const float* bias_dev,
                       void* out, int out_pitch, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res);
 int tf32_split_weights(const float* w, size_t count, float* dst);
+// a 16-bit DWPW stage as two steps (fd_conv_tc.cu): the depthwise half into the stage's intermediate, the pointwise half as a
+// 1x1 step of conv_tc_kernel; and the plan the block kernel would run the stage with (fd_block_tc.cu)
+bool pw_tc_supported(int dtype, const StageGeom& g);
+int pw_tc_prepare(int dtype, const StageGeom& g, const void* mid, const void* w, const float* scale_dev, const float* bias_dev,
+                  void* out, int out_pitch, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res);
+int dw_mid_launch(int dtype, const BlockArgs& a, cudaStream_t st);
+BlockPlanOut block_tc_plan_for(const StageGeom& g, const TcLaunchOpts& opts, bool* pinned);
 // device memory a kernel plan holds: its packed / padded parameter copies
 size_t block_tc_param_bytes(BlockTcPlan* bp);
 size_t chain_tc_param_bytes(ChainTcPlan* cp);
@@ -155,6 +163,7 @@ struct fd_plan {
     int opt_chain = 1;
     int opt_cluster = 1;
     int opt_tf32x3 = 0;
+    int opt_unfuse = 1;
     size_t workspace_bytes = 0;
     size_t split_bytes = 0;              // device memory of the stages' split weights (tf32x3), freed with the step sets
     // fd_pipeline_*: host batches flow H2D -> forward -> D2H through kPipeSlots device slots on three streams
@@ -177,6 +186,8 @@ struct fd_plan {
     int graph_misses = 0;                // consecutive fd_forward calls that found no captured graph for their (x, y) pair
 };
 static const size_t kMaxGraphs = 8;
+// the automatic two-step route is for stages whose depthwise intermediate stays in the 50 MB L2 between its two steps
+static const size_t kUnfuseMaxMidBytes = size_t(16) << 20;
 static const size_t kMaxStepSets = 8;
 
 namespace fd {
@@ -439,6 +450,44 @@ static int build_steps(fd_plan* p, int n, StepSet* ss) {
             const int dtype = p->dtype;
             const bool fuse_head = folded_here && p->opt_path == 1 && block_tc_supported(dtype, a.g, true);
             bool use_tc = p->opt_path == 1 && block_tc_supported(dtype, a.g, false);
+            // ---- the two-step route (plan option "unfuse"): the depthwise half once into `mid`, then the pointwise half as a
+            // 1x1 step of conv_tc_kernel.  The block kernel holds an item's accumulator in registers, 128 output channels at
+            // most, and every output-channel split recomputes the depthwise half and reloads the halo tile; where it would
+            // split 8 ways or more, or hand the operand tiles around a tile-sharing cluster, the stage's map is small enough
+            // to stay in the L2 between the two steps and fusion costs more than it saves.  Same bits either way.
+            const bool add_in_place = a.skip != nullptr && p->opt_tma_epilogue && p->opt_inplace_skip;
+            if (use_tc && p->opt_unfuse && !folded_here && (a.skip == nullptr || add_in_place) && pw_tc_supported(dtype, a.g)) {
+                bool pinned = false;
+                const BlockPlanOut bpo = block_tc_plan_for(a.g, lopts, &pinned);
+                const size_t mid_bytes = (size_t)px_out * sg.c_in * dtype_size(dtype);
+                const bool wide = bpo.ok && (bpo.splits >= 8 || bpo.cs > 1) && mid_bytes <= kUnfuseMaxMidBytes;
+                if (!pinned && (p->opt_unfuse == 2 || wide)) {
+                    void* out = a.skip ? const_cast<void*>(a.skip) : a.out;         // a skip is added where it lies
+                    const int opitch = a.skip ? a.g.skip_pitch : a.g.out_pitch;
+                    if (a.skip) r.out_eff = out;
+                    int rc = pw_tc_prepare(dtype, a.g, a.mid, a.pw_w, a.pw_scale, a.pw_bias, out, opitch, a.skip ? 1 : 0, lopts, &r.ctc);
+                    if (rc != FD_OK) return rc;
+                    ss->bytes += conv_tc_param_bytes(r.ctc);
+                    Step d;
+                    d.stage = i;
+                    d.name = sg.ksize == 3 ? "dw_mid_kernel<3>" : "dw_mid_kernel<5>";
+                    d.macs = dw_macs;
+                    d.dw_macs = dw_macs;
+                    d.alg_bytes = (px_in + px_out) * sg.c_in * es + (double)sg.c_in * (sg.ksize * sg.ksize + 2) * 4;
+                    d.run = [a, dtype](cudaStream_t stream, const void*, void*) { return dw_mid_launch(dtype, a, stream); };
+                    ss->steps.push_back(d);
+                    Step q;
+                    q.stage = i;
+                    q.name = std::string("pw:") + conv_tc_name(r.ctc);      // the pointwise half of a DWPW stage, not a CONV stage
+                    q.macs = pw_macs;
+                    q.alg_bytes = (px_out * sg.c_in + px_out * up * sg.c_out * (a.skip ? 2.0 : 1.0)) * es +
+                                  (double)sg.c_in * sg.c_out * es + 2.0 * sg.c_out * 4;
+                    ConvTcPlan* ctc = r.ctc;
+                    q.run = [ctc](cudaStream_t stream, const void*, void*) { return conv_tc_launch(ctc, stream); };
+                    ss->steps.push_back(q);
+                    continue;
+                }
+            }
             if (use_tc) {
                 // decoder blocks with a skip accumulate INTO the skip tensor (TMA reduce-add): that buffer becomes the
                 // block's output and the skip never has to be read by the SM
@@ -742,6 +791,7 @@ static int* option_slot(fd_plan* p, const char* name) {
     if (!strcmp(name, "chain")) return &p->opt_chain;
     if (!strcmp(name, "cluster")) return &p->opt_cluster;
     if (!strcmp(name, "tf32x3")) return &p->opt_tf32x3;
+    if (!strcmp(name, "unfuse")) return &p->opt_unfuse;
     return nullptr;
 }
 
@@ -749,8 +799,11 @@ int fd_plan_set_option(fd_plan* p, const char* name, int value) {
     int* slot = option_slot(p, name);
     if (!slot) return fail(FD_ERR_INVALID, std::string("unknown option: ") + (name ? name : "(null)"));
     const bool is_time = !strcmp(name, "wait_sleep_ns");
-    if (is_time ? (value < 0 || value > 100000) : (value != 0 && value != 1))
+    if (!strcmp(name, "unfuse")) {
+        if (value < 0 || value > 2) return fail(FD_ERR_INVALID, "unfuse must be 0, 1 or 2");
+    } else if (is_time ? (value < 0 || value > 100000) : (value != 0 && value != 1)) {
         return fail(FD_ERR_INVALID, is_time ? "wait_sleep_ns must be in [0, 100000]" : "option value must be 0 or 1");
+    }
     if (*slot != value) { *slot = value; invalidate(p); }
     return FD_OK;
 }
@@ -1087,6 +1140,15 @@ int fd_debug_conv_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_o
     const ConvPlanOut q = conv_tc_debug_plan(FD_STAGE_CONV, ksize, h_out, w_out, n, c_in, c_out, n_sms);
     const int v[16] = {q.ok, q.ni, q.th, q.tw, q.bn, q.stages, q.m_tiles, q.n_splits, q.items, q.waves, q.kblocks, q.smem_bytes,
                        q.useful_permille, (int)(q.cost > 2e9 ? 2e9 : q.cost), 0, 0};
+    for (int i = 0; i < 16; ++i) out[i] = v[i];
+    return FD_OK;
+}
+
+int fd_debug_pw_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms, int* out, int cap) {
+    if (!out || cap < 16) return fail(FD_ERR_INVALID, "need an int[16] output");
+    const ConvPlanOut q = pw_tc_debug_plan(h_out, w_out, n, c_in, c_out, upsample, n_sms);
+    const int v[16] = {q.ok, q.ni, q.th, q.tw, q.bn, q.stages, q.m_tiles, q.n_splits, q.items, q.waves, q.kblocks, q.smem_bytes,
+                       q.useful_permille, (int)(q.cost > 2e9 ? 2e9 : q.cost), q.ok ? conv_stage_bytes(q.bn) : 0, 0};
     for (int i = 0; i < 16; ++i) out[i] = v[i];
     return FD_OK;
 }

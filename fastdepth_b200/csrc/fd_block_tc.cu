@@ -917,6 +917,33 @@ static int block_wmc_auto(const StageGeom& g, const BlockPlanOut& po, int n_tile
     return 1;
 }
 
+// what the planner is asked for a block: its geometry, the plan's options and the environment's experiment knobs
+static BlockPlanIn block_plan_in(const StageGeom& g, int tile, int halfk, int n_tiles, int head, const TcLaunchOpts& opts) {
+    BlockPlanIn pin{};
+    pin.ksize = g.ksize; pin.stride = g.stride; pin.tile = tile; pin.c_in = g.c_in; pin.c_out = g.c_out; pin.n_tiles = n_tiles;
+    pin.head = head; pin.barrier_bytes = (int)sizeof(TcBarriers); pin.n_sms = opts.n_sms;
+    pin.cluster = (opts.cluster && !halfk) ? 0 : 1;
+    { const char* e = getenv("FD_TC_DW_TEAMS"); pin.even_rings = (e && *e == '1') ? 0 : ((e && *e == '2') ? 1 : 2); }   // 1 = never, 2 = wherever even rings fit
+    if (pin.even_rings == 2 && g.ksize == 5 && (g.c_in + TC_KBLK - 1) / TC_KBLK <= 2) pin.even_rings = 1;   // 5x5 blocks of <= 2 K-blocks
+    plan_env_knobs(pin);
+    if (halfk) pin.cluster = 1;
+    return pin;
+}
+
+// The plan block_tc_prepare would build for this (unfolded) block, without building it.  *pinned: an experiment knob of the
+// environment asks for a particular block-kernel plan (FD_TC_MAX_NCTA, FD_TC_CLUSTER >= 2, FD_TC_WMC, FD_TC_DW_TEAMS).
+BlockPlanOut block_tc_plan_for(const StageGeom& g, const TcLaunchOpts& opts, bool* pinned) {
+    const int tile = pick_tile(g);
+    const int NI = tile ? 2 : 1, TW = tile ? 8 : 16;
+    const int n_tiles = ((g.w_out + TW - 1) / TW) * ((g.h_out + 7) / 8) * ((g.n + NI - 1) / NI);
+    const char* e = getenv("FD_TC_NO_HALFK");
+    const int halfk = (g.c_in <= 32 && g.ksize == 3 && g.stride == 1 && tile == 0 && !(e && *e == '1')) ? 1 : 0;
+    const BlockPlanIn pin = block_plan_in(g, tile, halfk, n_tiles, 0, opts);
+    auto set = [](const char* name) { const char* v = getenv(name); return v && *v; };
+    *pinned = pin.max_n_cta > 0 || pin.cluster >= 2 || set("FD_TC_WMC") || set("FD_TC_DW_TEAMS");
+    return plan_block(pin);
+}
+
 int block_tc_prepare(int dtype, const BlockArgs& a, const float* head_w, float head_scale, float head_bias, int head_act,
                      void* head_out, bool tma_epilogue, const TcLaunchOpts& opts, BlockTcPlan** out) {
     PFN_encodeTiled encode = get_encode();
@@ -945,15 +972,7 @@ int block_tc_prepare(int dtype, const BlockArgs& a, const float* head_w, float h
     p.out_pitch = g.out_pitch > 0 ? g.out_pitch : g.c_out; p.skip_pitch = g.skip_pitch > 0 ? g.skip_pitch : g.c_out;
     const int in_pitch = g.in_pitch > 0 ? g.in_pitch : g.c_in;
 
-    BlockPlanIn pin{};
-    pin.ksize = g.ksize; pin.stride = g.stride; pin.tile = bp->tile; pin.c_in = g.c_in; pin.c_out = g.c_out; pin.n_tiles = n_tiles;
-    pin.head = p.head; pin.barrier_bytes = (int)sizeof(TcBarriers); pin.n_sms = opts.n_sms;
-    pin.cluster = (opts.cluster && !bp->halfk) ? 0 : 1;
-    { const char* e = getenv("FD_TC_DW_TEAMS"); pin.even_rings = (e && *e == '1') ? 0 : ((e && *e == '2') ? 1 : 2); }   // 1 = never, 2 = wherever even rings fit
-    if (pin.even_rings == 2 && g.ksize == 5 && (g.c_in + TC_KBLK - 1) / TC_KBLK <= 2) pin.even_rings = 1;   // 5x5 blocks of <= 2 K-blocks
-    plan_env_knobs(pin);
-    if (bp->halfk) pin.cluster = 1;
-    const BlockPlanOut po = plan_block(pin);
+    const BlockPlanOut po = plan_block(block_plan_in(g, bp->tile, bp->halfk, n_tiles, p.head, opts));
     if (!po.ok) { delete bp; return fail(FD_ERR_UNSUPPORTED, "fused block does not fit shared memory"); }
     const int splits = po.splits;
     p.n_cta = po.n_cta; p.splits = po.splits; p.items = po.items;

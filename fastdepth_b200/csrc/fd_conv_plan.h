@@ -97,6 +97,16 @@ struct ConvPlanOut {
 constexpr int kConvTiles[][3] = {{1, 8, 16}, {2, 8, 8}, {4, 4, 8}, {8, 4, 4}, {32, 2, 2}};
 constexpr int kConvNumTiles = 5;
 
+// A 1x1 conv without an upsample reads and writes rows of a matrix, M = n * h * w of them, and no box ever looks at a
+// neighbour: when 16 divides M the rows are presented as ONE image of M / 16 rows x 16 columns, so that 1 x 8 x 16 tiles cover
+// them with at most one partial tile (a 7x7 map in 2 x 8 x 8 boxes is 77 % used).  Returns false when the geometry stays.
+inline bool conv_flat_rows(int upsample, int* n, int* h, int* w) {
+    const long long m = (long long)*n * *h * *w;
+    if (upsample || m % 16 || m / 128 >= (1 << 18)) return false;     // (the kernel's item decode divides numbers below 2^20)
+    *n = 1; *h = (int)(m / 16); *w = 16;
+    return true;
+}
+
 inline int conv_stage_bytes(int bn) { return 128 * 128 + bn * 128; }
 // the split-TF32 pointwise instance: A {32 fp32 ch x 128 px} + B high + B low {32 fp32 ch x bn}
 inline int conv_stage_bytes_tf32x3(int bn) { return 128 * 128 + 2 * bn * 128; }

@@ -32,11 +32,18 @@
 // through view q.  It is a sibling kernel rather than an instance of conv_tc_kernel: producer, K loop and epilogue all
 // differ (two B boxes, A through registers, three MMAs per step, fp32 stores or reduce-adds), and the 16-bit instances stay
 // exactly as they were.
+//
+// A 16-bit DWPW stage that the fused block kernel would have to split many ways (plan option "unfuse", fd_api.cu) runs as two
+// steps instead: dw_mid_kernel writes the depthwise half once, to the stage's intermediate, and conv_tc_kernel runs the
+// pointwise half as a 1x1 CONV over it (one phase, one tap, the stage's own [c_out][c_in] weights; reduce = 1 adds the tiles
+// into the skip tensor with the TMA reduce-add).  The two steps compute what block_tc_kernel computes, bit for bit: the same
+// exact products in the same (ky, kx) order, the same k16 MMA sequence per accumulator, the same affine, act and rounding.
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
 #include <new>
 #include <string>
+#include <type_traits>
 
 #include "fd_conv_plan.h"
 #include "fd_tc_common.cuh"
@@ -85,7 +92,7 @@ __global__ void __launch_bounds__(CV_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w,
                const __grid_constant__ CUtensorMap tm_o0, const __grid_constant__ CUtensorMap tm_o1,
                const __grid_constant__ CUtensorMap tm_o2, const __grid_constant__ CUtensorMap tm_o3,
-               const __grid_constant__ ConvParams p) {
+               const __grid_constant__ ConvParams p, const int reduce) {
     using MF = MixFma<T>;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -193,11 +200,20 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
                     if (elected) {
                         const uint32_t src = smem_u32(stg);
                         const int cc = c.n0 + cb * 64;
-                        tma_store_4d(q == 0 ? &tm_o0 : q == 1 ? &tm_o1 : q == 2 ? &tm_o2 : &tm_o3, src, cc, c.ox0, c.oy0, c.img0);
-                        if (p.upsample) {
-                            tma_store_4d(&tm_o1, src, cc, c.ox0, c.oy0, c.img0);
-                            tma_store_4d(&tm_o2, src, cc, c.ox0, c.oy0, c.img0);
-                            tma_store_4d(&tm_o3, src, cc, c.ox0, c.oy0, c.img0);
+                        if (reduce) {      // a 1x1 step with a skip: the views already hold the skip tensor (never phased)
+                            tma_reduce_add_4d(&tm_o0, src, cc, c.ox0, c.oy0, c.img0);
+                            if (p.upsample) {
+                                tma_reduce_add_4d(&tm_o1, src, cc, c.ox0, c.oy0, c.img0);
+                                tma_reduce_add_4d(&tm_o2, src, cc, c.ox0, c.oy0, c.img0);
+                                tma_reduce_add_4d(&tm_o3, src, cc, c.ox0, c.oy0, c.img0);
+                            }
+                        } else {
+                            tma_store_4d(q == 0 ? &tm_o0 : q == 1 ? &tm_o1 : q == 2 ? &tm_o2 : &tm_o3, src, cc, c.ox0, c.oy0, c.img0);
+                            if (p.upsample) {
+                                tma_store_4d(&tm_o1, src, cc, c.ox0, c.oy0, c.img0);
+                                tma_store_4d(&tm_o2, src, cc, c.ox0, c.oy0, c.img0);
+                                tma_store_4d(&tm_o3, src, cc, c.ox0, c.oy0, c.img0);
+                            }
                         }
                         bulk_commit_group();
                     }
@@ -352,6 +368,84 @@ conv_tc_tf32x3_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_co
     }
 }
 
+// The depthwise half of a 16-bit DWPW stage on its own: k x k taps (stride 1 or 2) + fp32 affine + act, one rounding to 16
+// bits, NHWC in (in_pitch elements per pixel) -> dense NHWC mid.  One thread per PX neighbouring outputs of a row and 8
+// channels.  It follows block_tc_kernel's depthwise warps step by step: taps rounded to the storage dtype (as pack_dwp_kernel does), inputs and
+// taps widened to fp32, one fp32 FMA per tap with ky outer and kx inner, then ffma2_abc + pack_act.  The block kernel also
+// adds the zero-filled taps outside the map; skipping them is the same, since an accumulator that starts at +0 never becomes
+// -0 under round-to-nearest and x + 0 == x otherwise.
+template <typename T, int K, bool RELU6, int PX>
+__global__ void __launch_bounds__(256)
+dw_mid_kernel(const T* __restrict__ in, T* __restrict__ mid, const float* __restrict__ w, const float* __restrict__ scale,
+              const float* __restrict__ bias, int n, int h_in, int w_in, int h_out, int w_out, int c, int in_pitch, int stride) {
+    using MF = MixFma<T>;
+    const int groups = c >> 3, segs = (w_out + PX - 1) / PX;
+    const long long total = (long long)n * h_out * segs * groups;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= total) return;
+    const int g = (int)(idx % groups);
+    long long t = idx / groups;
+    const int ox0 = (int)(t % segs) * PX;
+    const int oy = (int)((t / segs) % h_out);
+    const int img = (int)(t / ((long long)segs * h_out));
+    constexpr int PAD = (K - 1) / 2;
+    auto rt = [](float v) { return Traits<T>::to_f(Traits<T>::from_f(v)); };
+    f32x2 acc[PX][4];
+#pragma unroll
+    for (int o = 0; o < PX; ++o)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[o][j] = 0ull;
+    const T* base = in + (size_t)img * h_in * w_in * in_pitch + g * 8;
+    // a thread owns PX neighbouring outputs of one row: every input pixel of a kernel row is loaded and widened once and
+    // feeds up to K of them; for each output the taps still arrive ky outer, kx inner (input column ascending)
+    auto row = [&](auto stride_c, int ky) {
+        constexpr int S = decltype(stride_c)::value;
+        const int iy = oy * S - PAD + ky;
+        if (iy < 0 || iy >= h_in) return;
+        f32x2 wk[K][4];
+#pragma unroll
+        for (int kx = 0; kx < K; ++kx) {
+            const float4* wp = reinterpret_cast<const float4*>(w + (size_t)(ky * K + kx) * c + g * 8);
+            const float4 w0 = __ldg(wp), w1 = __ldg(wp + 1);
+            wk[kx][0] = f32x2_make(rt(w0.x), rt(w0.y)); wk[kx][1] = f32x2_make(rt(w0.z), rt(w0.w));
+            wk[kx][2] = f32x2_make(rt(w1.x), rt(w1.y)); wk[kx][3] = f32x2_make(rt(w1.z), rt(w1.w));
+        }
+#pragma unroll
+        for (int j = 0; j < (PX - 1) * S + K; ++j) {
+            const int ix = ox0 * S - PAD + j;
+            if (ix < 0 || ix >= w_in) continue;
+            const uint4 v = __ldg(reinterpret_cast<const uint4*>(base + ((size_t)iy * w_in + ix) * in_pitch));
+            const f32x2 x0 = MF::widen(v.x), x1 = MF::widen(v.y), x2 = MF::widen(v.z), x3 = MF::widen(v.w);
+#pragma unroll
+            for (int o = 0; o < PX; ++o) {
+                const int kx = j - o * S;
+                if (kx < 0 || kx >= K) continue;
+                ffma2(acc[o][0], x0, wk[kx][0]); ffma2(acc[o][1], x1, wk[kx][1]);
+                ffma2(acc[o][2], x2, wk[kx][2]); ffma2(acc[o][3], x3, wk[kx][3]);
+            }
+        }
+    };
+#pragma unroll
+    for (int ky = 0; ky < K; ++ky) {
+        if (stride == 1) row(std::integral_constant<int, 1>(), ky);
+        else row(std::integral_constant<int, 2>(), ky);
+    }
+    const float4* sp = reinterpret_cast<const float4*>(scale + g * 8);
+    const float4* bp = reinterpret_cast<const float4*>(bias + g * 8);
+    const float4 s0 = __ldg(sp), s1 = __ldg(sp + 1), b0 = __ldg(bp), b1 = __ldg(bp + 1);
+    T* orow = mid + (((size_t)img * h_out + oy) * w_out) * c + g * 8;
+#pragma unroll
+    for (int o = 0; o < PX; ++o) {
+        if (ox0 + o >= w_out) break;
+        uint4 r;
+        r.x = MF::template pack_act<RELU6>(ffma2_abc(acc[o][0], f32x2_make(s0.x, s0.y), f32x2_make(b0.x, b0.y)));
+        r.y = MF::template pack_act<RELU6>(ffma2_abc(acc[o][1], f32x2_make(s0.z, s0.w), f32x2_make(b0.z, b0.w)));
+        r.z = MF::template pack_act<RELU6>(ffma2_abc(acc[o][2], f32x2_make(s1.x, s1.y), f32x2_make(b1.x, b1.y)));
+        r.w = MF::template pack_act<RELU6>(ffma2_abc(acc[o][3], f32x2_make(s1.z, s1.w), f32x2_make(b1.z, b1.w)));
+        *reinterpret_cast<uint4*>(orow + (size_t)(ox0 + o) * c) = r;
+    }
+}
+
 // ----------------------------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------------------------
@@ -414,8 +508,8 @@ ConvPlanOut conv_tc_debug_plan(int kind, int ksize, int h_out, int w_out, int n,
 // FD_CONV_TILE=<index into kConvTiles> / FD_CONV_BN=64|128|256 / FD_CONV_PHASE_GROUP=1|2 (phases per item of a DECONV / UPCONV
 // stage) pin the planner's choice (tests: the result must not depend on it).  `kind` is kConvKind*; a DECONV / UPCONV stage
 // passes its input map as g.h_out / g.w_out (the conv resolution) and writes the 2x map through the four phase views.
-int conv_tc_prepare(int dtype, int kind, const StageGeom& g, const void* in, const void* w, const float* scale_dev,
-                    const float* bias_dev, void* out, const TcLaunchOpts& opts, ConvTcPlan** res) {
+static int conv_prepare(int dtype, int kind, const StageGeom& g, const void* in, const void* w, const float* scale_dev,
+                        const float* bias_dev, void* out, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res) {
     PFN_encodeTiled encode = get_tensor_map_encoder();
     if (!encode) return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     const bool phased = kind != kConvKindConv;
@@ -429,7 +523,7 @@ int conv_tc_prepare(int dtype, int kind, const StageGeom& g, const void* in, con
     if (!po.ok) return fail(FD_ERR_UNSUPPORTED, "dense conv stage: no tile plan fits shared memory");
     ConvTcPlan* cp = new (std::nothrow) ConvTcPlan();
     if (!cp) return fail(FD_ERR_CUDA, "out of host memory");
-    cp->dtype = dtype; cp->act = g.act; cp->opts = opts; cp->po = po;
+    cp->dtype = dtype; cp->act = g.act; cp->opts = opts; cp->po = po; cp->reduce = reduce;
     ConvParams& p = cp->p;
     memset(&p, 0, sizeof(p));
     p.n = g.n; p.h = g.h_out; p.w = g.w_out; p.c_in = g.c_in; p.c_out = g.c_out;
@@ -498,8 +592,8 @@ int conv_tc_prepare(int dtype, int kind, const StageGeom& g, const void* in, con
     cp->grid = dim3((unsigned)(p.items < opts.n_sms ? p.items : opts.n_sms), 1, 1);
     char buf[160];
     if (!phased)
-        snprintf(buf, sizeof(buf), "conv_tc_kernel<k%d,bn%d,%s>[%dx%dx%d,n%d,st%d,%s]", g.ksize, po.bn, g.upsample ? "up" : "noup",
-                 po.ni, po.th, po.tw, p.splits, p.stages, g.act == FD_ACT_RELU6 ? "relu6" : "relu");
+        snprintf(buf, sizeof(buf), "conv_tc_kernel<k%d,bn%d,%s>[%dx%dx%d,n%d,st%d,%s%s]", g.ksize, po.bn, g.upsample ? "up" : "noup",
+                 po.ni, po.th, po.tw, p.splits, p.stages, g.act == FD_ACT_RELU6 ? "relu6" : "relu", reduce ? ",+skip(red)" : "");
     else   // 4ph: one phase per item; 4ph2: the diagonal phase pairs
         snprintf(buf, sizeof(buf), "conv_tc_kernel<%s%d,bn%d,%s>[%dx%dx%d,n%d,st%d,%s]", kind == kConvKindDeconv ? "deconv" : "upconv",
                  g.ksize, po.bn, po.groups == 2 ? "4ph2" : "4ph", po.ni, po.th, po.tw, p.splits, p.stages,
@@ -507,6 +601,66 @@ int conv_tc_prepare(int dtype, int kind, const StageGeom& g, const void* in, con
     cp->name = buf;
     *res = cp;
     return FD_OK;
+}
+
+int conv_tc_prepare(int dtype, int kind, const StageGeom& g, const void* in, const void* w, const float* scale_dev,
+                    const float* bias_dev, void* out, const TcLaunchOpts& opts, ConvTcPlan** res) {
+    return conv_prepare(dtype, kind, g, in, w, scale_dev, bias_dev, out, 0, opts, res);
+}
+
+bool pw_tc_supported(int dtype, const StageGeom& g) {
+    if (dtype != FD_F16 && dtype != FD_BF16) return false;
+    return g.c_in % 8 == 0 && g.c_out % 8 == 0 && get_tensor_map_encoder() != nullptr;
+}
+
+// the 1x1 geometry of a DWPW stage's pointwise half: the dense intermediate in, rows of a matrix where nothing is upsampled
+static StageGeom pw_geom(const StageGeom& g, int out_pitch) {
+    StageGeom q = g;
+    q.ksize = 1; q.stride = 1;
+    conv_flat_rows(q.upsample, &q.n, &q.h_out, &q.w_out);
+    q.h_in = q.h_out; q.w_in = q.w_out; q.in_pitch = g.c_in; q.out_pitch = out_pitch;
+    return q;
+}
+
+ConvPlanOut pw_tc_debug_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms) {
+    ConvPlanIn q{};
+    q.ksize = 1; q.h_out = h_out; q.w_out = w_out; q.n = n; q.c_in = c_in; q.c_out = c_out; q.upsample = upsample;
+    q.n_sms = n_sms; q.force_tile = -1; q.kind = kConvKindConv;
+    conv_flat_rows(upsample, &q.n, &q.h_out, &q.w_out);
+    return plan_conv(q);
+}
+
+// The pointwise half of a 16-bit DWPW stage as a 1x1 step of conv_tc_kernel: `mid` is the stage's depthwise intermediate
+// (NHWC, c_in dense), `w` its pointwise weights [c_out][c_in]; `out` / `out_pitch` what the tiles are written to (g.upsample:
+// the four views of the 2x map).  reduce = 1: the tiles are reduce-added into `out`, which already holds the skip tensor.
+int pw_tc_prepare(int dtype, const StageGeom& g, const void* mid, const void* w, const float* scale_dev, const float* bias_dev,
+                  void* out, int out_pitch, int reduce, const TcLaunchOpts& opts, ConvTcPlan** res) {
+    return conv_prepare(dtype, kConvKindConv, pw_geom(g, out_pitch), mid, w, scale_dev, bias_dev, out, reduce, opts, res);
+}
+
+template <typename T, int PX>
+static int dw_mid_launch_t(const BlockArgs& a, cudaStream_t st) {
+    const StageGeom& g = a.g;
+    const long long total = (long long)g.n * g.h_out * ((g.w_out + PX - 1) / PX) * (g.c_in / 8);
+    const unsigned blocks = (unsigned)((total + 255) / 256);
+    const int in_pitch = g.in_pitch > 0 ? g.in_pitch : g.c_in;
+    const bool r6 = g.act == FD_ACT_RELU6;
+#define FD_DW_MID(K, R6)                                                                                                           \
+    dw_mid_kernel<T, K, R6, PX><<<blocks, 256, 0, st>>>(static_cast<const T*>(a.in), static_cast<T*>(a.mid), a.dw_w, a.dw_scale,  \
+                                                        a.dw_bias, g.n, g.h_in, g.w_in, g.h_out, g.w_out, g.c_in, in_pitch, g.stride)
+    if (g.ksize == 3) { if (r6) FD_DW_MID(3, true); else FD_DW_MID(3, false); }
+    else if (g.ksize == 5) { if (r6) FD_DW_MID(5, true); else FD_DW_MID(5, false); }
+    else return fail(FD_ERR_UNSUPPORTED, "no dw_mid_kernel instance for this kernel size");
+#undef FD_DW_MID
+    FD_CUDA_OK(cudaGetLastError());
+    return FD_OK;
+}
+
+// The depthwise half of a 16-bit DWPW stage into a.mid (see dw_mid_kernel).
+int dw_mid_launch(int dtype, const BlockArgs& a, cudaStream_t st) {
+    if (dtype != FD_F16 && dtype != FD_BF16) return fail(FD_ERR_UNSUPPORTED, "dw_mid_kernel is a 16-bit kernel");
+    // four outputs per thread: measured against one (more gathers) and eight (too few threads in flight), DESIGN 3.6a
+    return dtype == FD_F16 ? dw_mid_launch_t<__half, 4>(a, st) : dw_mid_launch_t<__nv_bfloat16, 4>(a, st);
 }
 
 bool pw_tf32x3_supported(const StageGeom& g) {
@@ -687,7 +841,8 @@ static int conv_launch_inst(ConvTcPlan* cp, cudaStream_t st) {
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = cp->opts.pdl ? 1 : 0;
-    FD_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, cp->tm_in, cp->tm_w, cp->tm_o[0], cp->tm_o[1], cp->tm_o[2], cp->tm_o[3], cp->p));
+    FD_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, cp->tm_in, cp->tm_w, cp->tm_o[0], cp->tm_o[1], cp->tm_o[2], cp->tm_o[3], cp->p,
+                                  cp->reduce));
     FD_CUDA_OK(cudaGetLastError());
     return FD_OK;
 }

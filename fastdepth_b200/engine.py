@@ -123,7 +123,7 @@ class ForwardLanes:
     """Throughput front end: ``lanes`` independent copies of the forward plan -- each with its own activation buffers, its own
     CUDA stream and its own C-ABI host pipeline (``fd_pipeline_submit`` / ``fd_pipeline_wait``) -- that take batches round-robin.
 
-    One forward is a chain of 15 persistent kernels with one 227 KB CTA per SM, so at every kernel boundary the SMs that finish early
+    One forward is a chain of 18 kernels, most of them persistent with one 227 KB CTA per SM, so at every kernel boundary the SMs that finish early
     idle until the next kernel has filled its pipeline.  A second and third batch in flight
     on other streams fill those gaps with their own kernels.
     The module's own ``forward`` keeps strict single-stream semantics (and the lowest latency); this class is for serving loops that

@@ -137,6 +137,15 @@ int fd_plan_set_stage_weights(fd_plan* plan, int stage,
  *                "chain" and "cluster" do not apply.  16-bit plans and path 0 ignore it.  fd_stage_buffer(which = 1)
  *                still returns the depthwise intermediate.  (fastdepth_b200.engine sets it from
  *                torch.get_float32_matmul_precision())  [default 0]
+ *   "unfuse"     a 16-bit DWPW stage on path 1 may run as two steps instead of the fused block kernel: dw_mid_kernel writes the
+ *                depthwise half once to the stage's intermediate, and conv_tc_kernel runs the pointwise half over it as a
+ *                1x1 conv (a skip is reduce-added in place).  The result is the fused kernel's, bit for bit.
+ *                0 = never; 1 = the stages the block planner would split 8 ways or more over the output channels, or run
+ *                on a tile-sharing cluster, and whose intermediate is at most 16 MB (stock b64 224x224: conv12, conv13,
+ *                decode_conv1); 2 = every DWPW stage the 1x1 step supports (not the block with the folded head, not a
+ *                stage inside a chain, a skip only with "tma_epilogue" and "inplace_skip").  A stage whose block-kernel
+ *                plan is pinned by FD_TC_MAX_NCTA, FD_TC_CLUSTER >= 2, FD_TC_WMC or FD_TC_DW_TEAMS stays fused.
+ *                fd_stage_buffer(which = 1) returns the intermediate of a two-step stage.  [default 1]
  *   "wait_sleep_ns" > 0: latency-tolerant roles of the fused block kernel (the TMA producer waiting for a
  *                free stage) sleep this many ns between barrier
  *                probes instead of spinning (the spinning waiters do not
@@ -174,12 +183,12 @@ int fd_pipeline_wait(fd_plan* plan, unsigned long long ticket);
 /* Introspection for stage-parity tests: the NHWC buffer stage `stage` wrote in the last
  * fd_forward (valid until the next one).  c_stride = elements between pixels.
  * which = 0: the stage output (after upsample/skip-add); 1: the depthwise intermediate
- * (only materialised on path 0; a CONV, DECONV or UPCONV stage has none and fails with FD_ERR_INVALID). */
+ * (only materialised on path 0 and by the two-step stages of "unfuse"; a CONV, DECONV or UPCONV stage has none and fails with FD_ERR_INVALID). */
 int fd_stage_buffer(fd_plan* plan, int stage, int which, void** dev_ptr,
                     int* n, int* h, int* w, int* c, int* c_stride);
 
 /* Bookkeeping used by bench.py.  A "step" is one kernel launch of fd_forward under the current
- * options (a DWPW stage is one fused step on path 1, a dw + a pw step on path 0); the step functions, fd_plan_time_steps,
+ * options (a DWPW stage is one fused step on path 1, or two under "unfuse"; a dw + a pw step on path 0); the step functions, fd_plan_time_steps,
  * fd_plan_trace_stage and fd_stage_buffer describe the steps of the plan's own N.  The workspace bytes include, once the
  * steps are built, the device memory they hold: with "tf32x3", the split weights [2][c_out][k*k][c_in] fp32 of every
  * split-TF32 step (once, shared by every batch size), and the packed parameter copies of every step set fd_forward_batch
@@ -231,6 +240,12 @@ int fd_debug_conv_plan(int ksize, int h_out, int w_out, int n, int c_in, int c_o
  * fd_debug_conv_plan, with kblocks counting 32-channel blocks (one 128-byte row of fp32); out[14] = bytes of one operand
  * stage (16 KB of A + 2 x bn x 128 B of B, the weights' high and low parts), out[15] = 0.  cap must be at least 16. */
 int fd_debug_pw_tf32x3_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms, int* out, int cap);
+
+/* Debug (host only, needs no GPU): the tile plan of the 16-bit pointwise step ("unfuse") of one DWPW stage on an h_out x w_out
+ * map.  Without an upsample the n * h_out * w_out rows are planned as one image of rows / 16 x 16 pixels when 16 divides
+ * them.  out[0..13] as in fd_debug_conv_plan (kblocks of 64 channels); out[14] = bytes of one operand stage (16 KB of A +
+ * bn x 128 B of B), out[15] = 0.  cap must be at least 16. */
+int fd_debug_pw_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms, int* out, int cap);
 
 int fd_debug_convt_plan(int kind, int ksize, int h_in, int w_in, int n, int c_in, int c_out, int n_sms, int* out, int cap);
 
