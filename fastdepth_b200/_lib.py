@@ -37,6 +37,7 @@ SIGNATURES = {
     'fd_plan_get_option': (ctypes.c_int, [_vp, ctypes.c_char_p, _c_int_p]),
     'fd_forward': (ctypes.c_int, [_vp, _vp, _vp, _vp]),
     'fd_forward_batch': (ctypes.c_int, [_vp, ctypes.c_int, _vp, _vp, _vp]),
+    'fd_forward_shape': (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]),
     'fd_forward_host': (ctypes.c_int, [_vp, _vp, _vp, _vp]),
     'fd_pipeline_submit': (ctypes.c_int, [_vp, _vp, _vp, ctypes.POINTER(ctypes.c_uint64)]),
     'fd_pipeline_wait': (ctypes.c_int, [_vp, ctypes.c_uint64]),

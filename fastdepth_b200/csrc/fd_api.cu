@@ -140,10 +140,18 @@ struct Step {
     std::function<int(cudaStream_t, const void*, void*)> run;
 };
 
-// The steps of a forward over images [0, n) of the plan's buffers.  Planner choices, grids, item counts and tensor maps
-// depend on n; the activation buffers, packed weights and split weights are the plan's and shared by every set.
+// The geometry of one stage in a forward of n images at h x w.
+struct StageShape {
+    StageGeom g{};
+    int out_h = 0, out_w = 0;            // spatial size of the stage's output buffer (after upsample)
+    int out_c = 0;                       // channels the NEXT stage sees (c_out, or c_out + c_skip after a concat)
+};
+
+// The steps of a forward of n images at h x w over the front of the plan's buffers.  Planner choices, grids, item counts
+// and tensor maps depend on (n, h, w); the activation buffers, packed weights and split weights are the plan's and shared
+// by every set.
 struct StepSet {
-    int n = 0;
+    int n = 0, h = 0, w = 0;
     std::vector<Step> steps;
     std::vector<StageRun> runs;          // per stage
     size_t bytes = 0;                    // device memory its kernel plans hold (packed parameter copies)
@@ -157,7 +165,7 @@ using namespace fd;
 struct fd_plan {
     int n = 0, h = 0, w = 0, dtype = 0, device = 0, n_sms = 132;
     std::vector<Stage> stages;
-    std::vector<StepSet*> sets;          // built lazily per live batch size; LRU-bounded, the set of the plan's own n is kept
+    std::vector<StepSet*> sets;          // built lazily per live (n, h, w); LRU-bounded, the set of the plan's own (N, H, W) is kept
     unsigned long long set_clock = 0;
     int opt_path = 1, opt_fold_head = 1, opt_graph = 1, opt_tma_epilogue = 1, opt_inplace_skip = 1, opt_pdl = 0, opt_wait_sleep_ns = 0;
     int opt_chain = 1;
@@ -178,9 +186,9 @@ struct fd_plan {
     bool last_stream_set = false;
     void* l2_flush = nullptr;
     size_t l2_flush_bytes = 0;
-    // CUDA graph cache keyed on the (x, y) pointer pair and the batch size: callers that rotate a few buffers (or let a
-    // caching allocator hand the same blocks back) replay; a new key is captured once, LRU-evicted.
-    struct GraphEntry { const void* x; void* y; int n; cudaGraphExec_t exec; unsigned long long stamp; };
+    // CUDA graph cache keyed on the (x, y) pointer pair and the shape (n, h, w): callers that rotate a few buffers (or let a
+    // caching allocator hand the same blocks back, possibly for another shape) replay; a new key is captured once, LRU-evicted.
+    struct GraphEntry { const void* x; void* y; int n, h, w; cudaGraphExec_t exec; unsigned long long stamp; };
     std::vector<GraphEntry> graphs;
     unsigned long long graph_clock = 0;
     int graph_misses = 0;                // consecutive fd_forward calls that found no captured graph for their (x, y) pair
@@ -208,6 +216,9 @@ static int dev_alloc(fd_plan* p, void** ptr, size_t bytes) {
     bytes = (bytes + 255) & ~size_t(255);
     FD_CUDA_OK(cudaMalloc(ptr, bytes));
     FD_CUDA_OK(cudaMemset(*ptr, 0, bytes));
+    // the fill runs on the legacy default stream, which the plan's non-blocking pipeline streams do not wait for: let it
+    // finish before one of them uploads into the buffer
+    FD_CUDA_OK(cudaStreamSynchronize(cudaStreamLegacy));
     p->workspace_bytes += bytes;
     return FD_OK;
 }
@@ -222,11 +233,14 @@ static void destroy_set(StepSet* ss) {
     delete ss;
 }
 
-static StepSet* find_set(fd_plan* p, int n) {
+static StepSet* find_set(fd_plan* p, int n, int h, int w) {
     for (StepSet* ss : p->sets)
-        if (ss->n == n) return ss;
+        if (ss->n == n && ss->h == h && ss->w == w) return ss;
     return nullptr;
 }
+
+// the set of the plan's own (N, H, W): never evicted, and the one the introspection functions describe
+static bool is_capacity_set(const fd_plan* p, const StepSet* ss) { return ss->n == p->n && ss->h == p->h && ss->w == p->w; }
 
 // weights or options changed: every step set, every graph and the split weights go
 static void invalidate(fd_plan* p) {
@@ -266,17 +280,93 @@ static int upload_as_dtype(int dtype, const float* host, size_t count, void* dev
     return FD_OK;
 }
 
-// Build the steps of a forward over images [0, n) into `ss`: every stage's geometry with n images, over the plan's buffers.
-static int build_steps(fd_plan* p, int n, StepSet* ss) {
+// Walk the stage list for a forward of n images at h x w: check every stage against its producer and return each stage's
+// geometry.  fd_plan_create sizes the plan's buffers from the walk at (N, H, W); every step set repeats it at its own shape.
+static int walk_stages(const fd_stage_desc* stages, int n_stages, int n, int h, int w, std::vector<StageShape>& out) {
+    out.assign(n_stages, StageShape());
+    std::vector<int> concat_src(n_stages, -1);         // >= 0: the stage's output is a channel slice of that stage's buffer
+    int ch = 3, hh = h, ww = w;
+    for (int i = 0; i < n_stages; ++i) {
+        const fd_stage_desc& d = stages[i];
+        StageShape& s = out[i];
+        const bool first = i == 0, lastst = i == n_stages - 1;
+        if ((d.kind == FD_STAGE_STEM) != first || (d.kind == FD_STAGE_HEAD) != lastst ||
+            (!first && !lastst && d.kind != FD_STAGE_DWPW && !is_conv(d.kind)))
+            return fail(FD_ERR_INVALID, "stage list must be STEM, (DWPW|CONV|DECONV|UPCONV)..., HEAD");
+        if (d.c_in != ch) return fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": c_in does not match producer");
+        if (d.act != FD_ACT_RELU && d.act != FD_ACT_RELU6) return fail(FD_ERR_INVALID, "bad act");
+        s.g.n = n; s.g.h_in = hh; s.g.w_in = ww; s.g.c_in = d.c_in; s.g.c_out = d.c_out;
+        s.g.ksize = d.ksize; s.g.stride = d.stride; s.g.act = d.act; s.g.upsample = d.upsample ? 1 : 0;
+        if (d.kind == FD_STAGE_STEM) {
+            if (d.ksize != 3 || d.c_in != 3 || d.c_out % 8 || d.stride < 1 || d.stride > 2 || d.upsample || d.skip_src >= 0)
+                return fail(FD_ERR_INVALID, "stem must be 3x3, c_in 3, c_out % 8 == 0, stride 1|2");
+            s.g.h_out = (hh + 2 - 3) / d.stride + 1; s.g.w_out = (ww + 2 - 3) / d.stride + 1;
+        } else if (d.kind == FD_STAGE_DWPW) {
+            if ((d.ksize != 3 && d.ksize != 5) || d.stride < 1 || d.stride > 2 || d.c_in % 8 || d.c_out % 8 || d.c_out <= 0)
+                return fail(FD_ERR_INVALID, "block stage needs k in {3,5}, stride 1|2, channels % 8 == 0");
+            const int pad = (d.ksize - 1) / 2;
+            s.g.h_out = (hh + 2 * pad - d.ksize) / d.stride + 1; s.g.w_out = (ww + 2 * pad - d.ksize) / d.stride + 1;
+        } else if (d.kind == FD_STAGE_CONV) {
+            if (d.skip_src >= 0) return fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": a CONV stage takes no skip");
+            if (d.stride != 1) return fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": a CONV stage has stride 1");
+            if ((d.ksize != 3 && d.ksize != 5) || d.c_in % 8 || d.c_out % 8 || d.c_out <= 0 || (d.upsample != 0 && d.upsample != 1))
+                return fail(FD_ERR_INVALID, "conv stage needs k in {3,5}, channels % 8 == 0, upsample 0|1");
+            s.g.h_out = hh; s.g.w_out = ww;
+        } else if (is_phased(d.kind)) {
+            const char* nm = d.kind == FD_STAGE_DECONV ? "a DECONV" : "an UPCONV";
+            if (d.skip_src >= 0) return fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": " + nm + " stage takes no skip");
+            if (d.stride != 2) return fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": " + nm + " stage has stride 2");
+            if (d.upsample != 0) return fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": " + nm + " stage has upsample 0");
+            const bool k_ok = d.kind == FD_STAGE_DECONV ? (d.ksize == 3 || d.ksize == 5 || d.ksize == 7 || d.ksize == 9) : d.ksize == 5;
+            if (!k_ok || d.c_in % 8 || d.c_out % 8 || d.c_out <= 0)
+                return fail(FD_ERR_INVALID, d.kind == FD_STAGE_DECONV ? "deconv stage needs k in {3,5,7,9}, channels % 8 == 0"
+                                                                      : "upconv stage needs k 5, channels % 8 == 0");
+            s.g.h_out = hh; s.g.w_out = ww;            // the phase convs run at the input resolution; the output is 2h x 2w
+        } else {
+            if (d.ksize != 1 || d.c_out != 1 || d.c_in % 8 || d.upsample || d.skip_src >= 0)
+                return fail(FD_ERR_INVALID, "head must be 1x1, c_out 1, c_in % 8 == 0");
+            s.g.h_out = hh; s.g.w_out = ww;
+        }
+        s.out_h = s.g.h_out * (s.g.upsample || is_phased(d.kind) ? 2 : 1);
+        s.out_w = s.g.w_out * (s.g.upsample || is_phased(d.kind) ? 2 : 1);
+        s.out_c = d.c_out;
+        if (d.skip_src >= 0) {
+            if (d.kind != FD_STAGE_DWPW || !d.upsample || d.skip_src >= i) return fail(FD_ERR_INVALID, "bad skip_src");
+            const StageShape& src = out[d.skip_src];
+            if (src.out_h != s.out_h || src.out_w != s.out_w || (!d.skip_mode && src.g.c_out != d.c_out))
+                return fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": skip tensor shape does not match the upsampled output");
+            if (d.skip_mode) {
+                // concatenation (models.py:806-811): the stage's output is one wide NHWC buffer [.., c_out + c_skip]
+                if (d.skip_mode != 1 || concat_src[d.skip_src] >= 0 || stages[d.skip_src].skip_src >= 0)
+                    return fail(FD_ERR_INVALID, "bad skip_mode / skip source");
+                s.out_c = d.c_out + src.g.c_out;
+                concat_src[d.skip_src] = i;
+            }
+        }
+        ch = s.out_c; hh = s.out_h; ww = s.out_w;
+    }
+    if (hh != h || ww != w) return fail(FD_ERR_INVALID, "stage list does not return to the input resolution");
+    return FD_OK;
+}
+
+// Build the steps of a forward of n images at h x w into `ss`: every stage's geometry at that shape, over the front of the
+// plan's buffers.  Every decision that depends on the geometry (the chain kernel, the two-step route, the planners) is
+// taken from the set's own geometry, as a plan built for (n, h, w) takes it.
+static int build_steps(fd_plan* p, int n, int h, int w, StepSet* ss) {
     const int ns = (int)p->stages.size();
     const double es = (double)dtype_size(p->dtype);
     for (auto& s : p->stages)
         if (!s.have_weights) return fail(FD_ERR_STATE, "fd_plan_set_stage_weights was not called for every stage");
-    ss->n = n;
+    ss->n = n; ss->h = h; ss->w = w;
     ss->runs.assign(ns, StageRun());
     std::vector<StageRun>& R = ss->runs;
+    std::vector<fd_stage_desc> D(ns);
+    for (int i = 0; i < ns; ++i) D[i] = p->stages[i].d;
+    std::vector<StageShape> S;
+    int wrc = walk_stages(D.data(), ns, n, h, w, S);
+    if (wrc != FD_OK) return wrc;
     std::vector<StageGeom> G(ns);
-    for (int i = 0; i < ns; ++i) { G[i] = p->stages[i].g; G[i].n = n; }
+    for (int i = 0; i < ns; ++i) G[i] = S[i].g;
 
     TcLaunchOpts lopts;                   // every kernel plan keeps its own copy (no process-wide launch state)
     lopts.pdl = p->opt_pdl; lopts.sleep_ns = p->opt_wait_sleep_ns; lopts.n_sms = p->n_sms; lopts.cluster = p->opt_cluster;
@@ -493,7 +583,7 @@ static int build_steps(fd_plan* p, int n, StepSet* ss) {
                 // block's output and the skip never has to be read by the SM
                 const bool tma_epi = p->opt_tma_epilogue != 0;
                 if (tma_epi && p->opt_inplace_skip && a.skip != nullptr) { a.out = const_cast<void*>(a.skip); r.out_eff = a.out; }
-                int rc = fuse_head ? block_tc_prepare(dtype, a, head.pw_w_f32, head.head_scale, head.head_bias, head.g.act, nullptr, false, lopts, &r.tc)
+                int rc = fuse_head ? block_tc_prepare(dtype, a, head.pw_w_f32, head.head_scale, head.head_bias, G[ns - 1].act, nullptr, false, lopts, &r.tc)
                                    : block_tc_prepare(dtype, a, nullptr, 0.f, 0.f, 0, nullptr, tma_epi && (a.skip == nullptr || a.skip == a.out), lopts, &r.tc);
                 if (rc != FD_OK) return rc;
                 ss->bytes += block_tc_param_bytes(r.tc);
@@ -541,7 +631,7 @@ static int build_steps(fd_plan* p, int n, StepSet* ss) {
                     ConvTcPlan* ctc = r.ctc;
                     const bool copy = add && !inplace;
                     const void* skip = a.skip;
-                    const size_t rows = (size_t)a.g.n * s.out_h * s.out_w, row_bytes = (size_t)a.g.c_out * 4;
+                    const size_t rows = (size_t)a.g.n * S[i].out_h * S[i].out_w, row_bytes = (size_t)a.g.c_out * 4;
                     const size_t dpitch = (size_t)a.g.out_pitch * 4, spitch = (size_t)a.g.skip_pitch * 4;
                     q.run = [ctc, copy, out, skip, rows, row_bytes, dpitch, spitch](cudaStream_t stream, const void*, void*) {
                         if (copy)
@@ -555,7 +645,7 @@ static int build_steps(fd_plan* p, int n, StepSet* ss) {
             }
         } else if (!head_fused) {  // HEAD (unless decode_conv6 already ran inside the last block's epilogue)
             const bool up = fold;
-            const int hh = up ? last.g.h_out : sg.h_in, ww = up ? last.g.w_out : sg.w_in;
+            const int hh = up ? G[ns - 2].h_out : sg.h_in, ww = up ? G[ns - 2].w_out : sg.w_in;
             const long long m_total = (long long)sg.n * hh * ww;
             Step st;
             st.stage = i;
@@ -610,78 +700,30 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages, int n, int h, int 
     DeviceGuard guard(device);
     if (!guard.ok) return fail(FD_ERR_CUDA, "cudaSetDevice failed");
 
+    std::vector<StageShape> shapes;
+    int rc = walk_stages(stages, n_stages, n, h, w, shapes);
+    if (rc != FD_OK) return rc;
+
     fd_plan* p = new fd_plan();
     p->n = n; p->h = h; p->w = w; p->dtype = dtype; p->device = device; p->n_sms = prop.multiProcessorCount;
     p->stages.resize(n_stages);
     const size_t es = dtype_size(dtype);
-    int ch = 3, hh = h, ww = w;
-    int rc = FD_OK;
-    for (int i = 0; i < n_stages && rc == FD_OK; ++i) {
+    for (int i = 0; i < n_stages; ++i) {
         Stage& s = p->stages[i];
         s.d = stages[i];
         const fd_stage_desc& d = s.d;
-        const bool first = i == 0, lastst = i == n_stages - 1;
-        if ((d.kind == FD_STAGE_STEM) != first || (d.kind == FD_STAGE_HEAD) != lastst ||
-            (!first && !lastst && d.kind != FD_STAGE_DWPW && !is_conv(d.kind))) {
-            rc = fail(FD_ERR_INVALID, "stage list must be STEM, (DWPW|CONV|DECONV|UPCONV)..., HEAD"); break; }
-        if (d.c_in != ch) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": c_in does not match producer"); break; }
-        if (d.act != FD_ACT_RELU && d.act != FD_ACT_RELU6) { rc = fail(FD_ERR_INVALID, "bad act"); break; }
-        s.g.n = n; s.g.h_in = hh; s.g.w_in = ww; s.g.c_in = d.c_in; s.g.c_out = d.c_out;
-        s.g.ksize = d.ksize; s.g.stride = d.stride; s.g.act = d.act; s.g.upsample = d.upsample ? 1 : 0;
-        if (d.kind == FD_STAGE_STEM) {
-            if (d.ksize != 3 || d.c_in != 3 || d.c_out % 8 || d.stride < 1 || d.stride > 2 || d.upsample || d.skip_src >= 0) {
-                rc = fail(FD_ERR_INVALID, "stem must be 3x3, c_in 3, c_out % 8 == 0, stride 1|2"); break; }
-            s.g.h_out = (hh + 2 - 3) / d.stride + 1; s.g.w_out = (ww + 2 - 3) / d.stride + 1;
-        } else if (d.kind == FD_STAGE_DWPW) {
-            if ((d.ksize != 3 && d.ksize != 5) || d.stride < 1 || d.stride > 2 || d.c_in % 8 || d.c_out % 8 || d.c_out <= 0) {
-                rc = fail(FD_ERR_INVALID, "block stage needs k in {3,5}, stride 1|2, channels % 8 == 0"); break; }
-            const int pad = (d.ksize - 1) / 2;
-            s.g.h_out = (hh + 2 * pad - d.ksize) / d.stride + 1; s.g.w_out = (ww + 2 * pad - d.ksize) / d.stride + 1;
-        } else if (d.kind == FD_STAGE_CONV) {
-            if (d.skip_src >= 0) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": a CONV stage takes no skip"); break; }
-            if (d.stride != 1) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": a CONV stage has stride 1"); break; }
-            if ((d.ksize != 3 && d.ksize != 5) || d.c_in % 8 || d.c_out % 8 || d.c_out <= 0 || (d.upsample != 0 && d.upsample != 1)) {
-                rc = fail(FD_ERR_INVALID, "conv stage needs k in {3,5}, channels % 8 == 0, upsample 0|1"); break; }
-            s.g.h_out = hh; s.g.w_out = ww;
-        } else if (is_phased(d.kind)) {
-            const char* nm = d.kind == FD_STAGE_DECONV ? "a DECONV" : "an UPCONV";
-            if (d.skip_src >= 0) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": " + nm + " stage takes no skip"); break; }
-            if (d.stride != 2) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": " + nm + " stage has stride 2"); break; }
-            if (d.upsample != 0) { rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": " + nm + " stage has upsample 0"); break; }
-            const bool k_ok = d.kind == FD_STAGE_DECONV ? (d.ksize == 3 || d.ksize == 5 || d.ksize == 7 || d.ksize == 9) : d.ksize == 5;
-            if (!k_ok || d.c_in % 8 || d.c_out % 8 || d.c_out <= 0) {
-                rc = fail(FD_ERR_INVALID, d.kind == FD_STAGE_DECONV ? "deconv stage needs k in {3,5,7,9}, channels % 8 == 0"
-                                                                    : "upconv stage needs k 5, channels % 8 == 0");
-                break; }
-            s.g.h_out = hh; s.g.w_out = ww;            // the phase convs run at the input resolution; the output is 2h x 2w
-        } else {
-            if (d.ksize != 1 || d.c_out != 1 || d.c_in % 8 || d.upsample || d.skip_src >= 0) {
-                rc = fail(FD_ERR_INVALID, "head must be 1x1, c_out 1, c_in % 8 == 0"); break; }
-            s.g.h_out = hh; s.g.w_out = ww;
-        }
-        s.out_h = s.g.h_out * (s.g.upsample || is_phased(d.kind) ? 2 : 1);
-        s.out_w = s.g.w_out * (s.g.upsample || is_phased(d.kind) ? 2 : 1);
-        s.out_c = d.c_out; s.out_pitch = d.c_out;
-        if (d.skip_src >= 0) {
-            if (d.kind != FD_STAGE_DWPW || !d.upsample || d.skip_src >= i) { rc = fail(FD_ERR_INVALID, "bad skip_src"); break; }
-            Stage& src = p->stages[d.skip_src];
-            if (src.out_h != s.out_h || src.out_w != s.out_w || (!d.skip_mode && src.g.c_out != d.c_out)) {
-                rc = fail(FD_ERR_INVALID, "stage " + std::to_string(i) + ": skip tensor shape does not match the upsampled output");
-                break; }
-            if (d.skip_mode) {
-                // concatenation (models.py:806-811): one wide NHWC buffer [.., c_out + c_skip]; this stage writes the channel
-                // slice [0, c_out), the skip source is re-pointed to write (and be read by its consumer) in slice [c_out, ..)
-                if (d.skip_mode != 1 || src.concat_src >= 0 || src.d.skip_src >= 0) { rc = fail(FD_ERR_INVALID, "bad skip_mode / skip source"); break; }
-                s.out_c = d.c_out + src.g.c_out; s.out_pitch = s.out_c;
-            }
-        }
+        s.g = shapes[i].g;
+        s.out_h = shapes[i].out_h; s.out_w = shapes[i].out_w;
+        s.out_c = shapes[i].out_c; s.out_pitch = s.out_c;
         if (d.kind != FD_STAGE_HEAD) {
             rc = dev_alloc(p, &s.out, (size_t)n * s.out_h * s.out_w * s.out_pitch * es);
             if (rc) break;
             s.out_alloc = s.out;
             if (d.skip_src >= 0 && d.skip_mode) {
+                // concatenation (models.py:806-811): one wide NHWC buffer [.., c_out + c_skip]; this stage writes the channel
+                // slice [0, c_out), the skip source is re-pointed to write (and be read by its consumer) in slice [c_out, ..).
+                // The source's own dense buffer stays allocated (freed with the plan) but is no longer used
                 Stage& src = p->stages[d.skip_src];
-                // the source's own dense buffer stays allocated (freed with the plan) but is no longer used
                 src.out = static_cast<char*>(s.out) + (size_t)d.c_out * es;
                 src.out_pitch = s.out_pitch;
                 src.concat_src = i;
@@ -702,9 +744,7 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages, int n, int h, int 
         }
         if ((rc = dev_alloc(p, (void**)&s.pw_scale, (size_t)d.c_out * 4))) break;
         if ((rc = dev_alloc(p, (void**)&s.pw_bias, (size_t)d.c_out * 4))) break;
-        ch = s.out_c; hh = s.out_h; ww = s.out_w;
     }
-    if (rc == FD_OK && (hh != h || ww != w)) rc = fail(FD_ERR_INVALID, "stage list does not return to the input resolution");
     if (rc != FD_OK) {
         std::string keep = g_last_error;
         fd_plan_destroy(p);
@@ -815,24 +855,29 @@ int fd_plan_get_option(fd_plan* p, const char* name, int* value) {
     return FD_OK;
 }
 
-// The step set for batch size n, built on first use.  Beyond kMaxStepSets the least recently used set goes, with its graphs;
-// the set of the plan's own n stays (introspection describes it).
-static int ensure_steps(fd_plan* p, int n, StepSet** out) {
-    StepSet* ss = find_set(p, n);
+// The step set for (n, h, w), built on first use.  Beyond kMaxStepSets the least recently used set goes, with its graphs;
+// the set of the plan's own (N, H, W) stays (introspection describes it).
+static int ensure_steps(fd_plan* p, int n, int h, int w, StepSet** out) {
+    StepSet* ss = find_set(p, n, h, w);
     if (!ss) {
         if (p->sets.size() >= kMaxStepSets) {
             size_t victim = p->sets.size();
             for (size_t i = 0; i < p->sets.size(); ++i)
-                if (p->sets[i]->n != p->n && (victim == p->sets.size() || p->sets[i]->stamp < p->sets[victim]->stamp)) victim = i;
-            const int vn = p->sets[victim]->n;
+                if (!is_capacity_set(p, p->sets[i]) && (victim == p->sets.size() || p->sets[i]->stamp < p->sets[victim]->stamp))
+                    victim = i;
+            const StepSet* v = p->sets[victim];
             for (size_t i = 0; i < p->graphs.size();)
-                if (p->graphs[i].n == vn) { cudaGraphExecDestroy(p->graphs[i].exec); p->graphs.erase(p->graphs.begin() + i); }
-                else ++i;
+                if (p->graphs[i].n == v->n && p->graphs[i].h == v->h && p->graphs[i].w == v->w) {
+                    cudaGraphExecDestroy(p->graphs[i].exec);
+                    p->graphs.erase(p->graphs.begin() + i);
+                } else {
+                    ++i;
+                }
             destroy_set(p->sets[victim]);
             p->sets.erase(p->sets.begin() + victim);
         }
         ss = new StepSet();
-        int rc = build_steps(p, n, ss);
+        int rc = build_steps(p, n, h, w, ss);
         if (rc != FD_OK) { destroy_set(ss); return rc; }
         p->sets.push_back(ss);
     }
@@ -845,18 +890,33 @@ static int forward_enqueue(fd_plan* p, const StepSet* ss, const void* x_dev, voi
 
 int fd_forward(fd_plan* p, const void* x_dev, void* y_dev, void* stream) {
     if (!p) return fail(FD_ERR_INVALID, "NULL argument");
-    return fd_forward_batch(p, p->n, x_dev, y_dev, stream);
+    return fd_forward_shape(p, p->n, p->h, p->w, x_dev, y_dev, stream);
 }
 
 int fd_forward_batch(fd_plan* p, int n, const void* x_dev, void* y_dev, void* stream) {
     if (!p) return fail(FD_ERR_INVALID, "NULL argument");
-    if (n < 1 || n > p->n)
-        return fail(FD_ERR_INVALID, "batch size " + std::to_string(n) + " is outside [1, " + std::to_string(p->n) +
-                                        "], the plan's batch capacity");
+    return fd_forward_shape(p, n, p->h, p->w, x_dev, y_dev, stream);
+}
+
+int fd_forward_shape(fd_plan* p, int n, int h, int w, const void* x_dev, void* y_dev, void* stream) {
+    if (!p) return fail(FD_ERR_INVALID, "NULL argument");
+    if (h <= 0 || w <= 0 || h % 32 || w % 32)
+        return fail(FD_ERR_INVALID, "h and w must be positive multiples of 32, got " + std::to_string(h) + "x" + std::to_string(w));
+    // every stage buffer is dense NHWC of n * (h/s) * (w/s) * C elements, so any (n, h, w) with n*h*w <= N*H*W fits in its front
+    const long long cap = (long long)p->n * p->h * p->w, per_image = (long long)h * w;
+    const std::string plan_shape = std::to_string(p->n) + " x " + std::to_string(p->h) + " x " + std::to_string(p->w);
+    if (per_image > cap)
+        return fail(FD_ERR_INVALID, std::to_string(h) + "x" + std::to_string(w) + " needs " + std::to_string(per_image) +
+                                        " pixels per image, more than the plan's capacity of " + std::to_string(cap) +
+                                        " pixels (N x H x W = " + plan_shape + ")");
+    if (n < 1 || n > cap / per_image)
+        return fail(FD_ERR_INVALID, "batch size " + std::to_string(n) + " is outside [1, " + std::to_string(cap / per_image) +
+                                        "] at " + std::to_string(h) + "x" + std::to_string(w) + ": the plan's capacity is " +
+                                        std::to_string(cap) + " pixels (N x H x W = " + plan_shape + ")");
     if (!x_dev || !y_dev) return fail(FD_ERR_INVALID, "NULL argument");
     DeviceGuard guard(p->device);
     StepSet* ss = nullptr;
-    int rc = ensure_steps(p, n, &ss);
+    int rc = ensure_steps(p, n, h, w, &ss);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     // A plan owns ONE set of activation buffers: a forward enqueued on another stream than the previous one first waits for that
@@ -878,9 +938,9 @@ static int forward_enqueue(fd_plan* p, const StepSet* ss, const void* x_dev, voi
     int rc = FD_OK;
     if (!p->opt_graph) return run_steps(ss, x_dev, y_dev, st);
 
-    // Replay from a CUDA graph captured for this (x, y, n).
+    // Replay from a CUDA graph captured for this (x, y, n, h, w).
     for (auto& g : p->graphs)
-        if (g.x == x_dev && g.y == y_dev && g.n == ss->n) {
+        if (g.x == x_dev && g.y == y_dev && g.n == ss->n && g.h == ss->h && g.w == ss->w) {
             g.stamp = ++p->graph_clock;
             p->graph_misses = 0;
             FD_CUDA_OK(cudaGraphLaunch(g.exec, st));
@@ -914,7 +974,7 @@ static int forward_enqueue(fd_plan* p, const StepSet* ss, const void* x_dev, voi
         cudaGraphExecDestroy(p->graphs[victim].exec);
         p->graphs.erase(p->graphs.begin() + victim);
     }
-    p->graphs.push_back({x_dev, y_dev, ss->n, exec, ++p->graph_clock});
+    p->graphs.push_back({x_dev, y_dev, ss->n, ss->h, ss->w, exec, ++p->graph_clock});
     FD_CUDA_OK(cudaGraphLaunch(exec, st));
     return FD_OK;
 }
@@ -998,7 +1058,7 @@ int fd_pipeline_wait(fd_plan* p, unsigned long long ticket) {
 int fd_stage_buffer(fd_plan* p, int stage, int which, void** dev_ptr, int* n, int* h, int* w, int* c, int* c_stride) {
     if (!p || stage < 0 || stage >= (int)p->stages.size() || !dev_ptr) return fail(FD_ERR_INVALID, "bad argument");
     Stage& s = p->stages[stage];
-    const StepSet* full = find_set(p, p->n);
+    const StepSet* full = find_set(p, p->n, p->h, p->w);
     int hh, ww, cc;
     void* ptr;
     if (which == 0) {
@@ -1025,7 +1085,7 @@ int fd_plan_launches_per_forward(fd_plan* p, int* n_launches) {
     if (!p || !n_launches) return fail(FD_ERR_INVALID, "NULL argument");
     DeviceGuard guard(p->device);
     StepSet* ss = nullptr;
-    int rc = ensure_steps(p, p->n, &ss);
+    int rc = ensure_steps(p, p->n, p->h, p->w, &ss);
     if (rc) return rc;
     *n_launches = (int)ss->steps.size();
     return FD_OK;
@@ -1033,10 +1093,10 @@ int fd_plan_launches_per_forward(fd_plan* p, int* n_launches) {
 
 int fd_plan_workspace_bytes(fd_plan* p, size_t* bytes) {
     if (!p || !bytes) return fail(FD_ERR_INVALID, "NULL argument");
-    // the packed parameter copies of the plan's own step set are not counted; every smaller batch's set adds its own
+    // the packed parameter copies of the plan's own step set are not counted; every other (n, h, w)'s set adds its own
     size_t sets = 0;
     for (const StepSet* ss : p->sets)
-        if (ss->n != p->n) sets += ss->bytes;
+        if (!is_capacity_set(p, ss)) sets += ss->bytes;
     *bytes = p->workspace_bytes + p->split_bytes + sets;
     return FD_OK;
 }
@@ -1047,7 +1107,7 @@ int fd_plan_step_info(fd_plan* p, int step, int* stage, double* alg_bytes, doubl
     if (!p) return fail(FD_ERR_INVALID, "NULL plan");
     DeviceGuard guard(p->device);
     StepSet* ss = nullptr;
-    int rc = ensure_steps(p, p->n, &ss);
+    int rc = ensure_steps(p, p->n, p->h, p->w, &ss);
     if (rc) return rc;
     if (step < 0 || step >= (int)ss->steps.size()) return fail(FD_ERR_INVALID, "bad step index");
     const Step& s = ss->steps[step];
@@ -1065,7 +1125,7 @@ int fd_plan_step_macs(fd_plan* p, int step, double* dw_macs, double* dense_macs)
     if (!p) return fail(FD_ERR_INVALID, "NULL plan");
     DeviceGuard guard(p->device);
     StepSet* ss = nullptr;
-    int rc = ensure_steps(p, p->n, &ss);
+    int rc = ensure_steps(p, p->n, p->h, p->w, &ss);
     if (rc) return rc;
     if (step < 0 || step >= (int)ss->steps.size()) return fail(FD_ERR_INVALID, "bad step index");
     const Step& s = ss->steps[step];
@@ -1079,7 +1139,7 @@ int fd_plan_time_steps(fd_plan* p, const void* x_dev, void* y_dev, void* stream,
     if (!p || !x_dev || !y_dev || !ms_out || iters <= 0) return fail(FD_ERR_INVALID, "bad argument");
     DeviceGuard guard(p->device);
     StepSet* ss = nullptr;
-    int rc = ensure_steps(p, p->n, &ss);
+    int rc = ensure_steps(p, p->n, p->h, p->w, &ss);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (flush_l2 && !p->l2_flush) {
@@ -1116,7 +1176,7 @@ int fd_plan_trace_stage(fd_plan* p, int stage, void* y_dev, void* stream, unsign
     if (!p || stage < 0 || stage >= (int)p->stages.size() || !out_host || !rows || !cols) return fail(FD_ERR_INVALID, "bad argument");
     DeviceGuard guard(p->device);
     StepSet* ss = nullptr;
-    int rc = ensure_steps(p, p->n, &ss);
+    int rc = ensure_steps(p, p->n, p->h, p->w, &ss);
     if (rc) return rc;
     if (cap < 12 * 256) return fail(FD_ERR_INVALID, "trace buffer too small (need 3072 entries)");
     if (is_conv(p->stages[stage].d.kind)) return fail(FD_ERR_INVALID, "the stage timeline exists for fused block kernels only");

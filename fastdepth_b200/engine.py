@@ -11,10 +11,12 @@ under the default ``'highest'`` they stay on the fp32 SIMT kernels.  An explicit
 precision setting.  ``models.MobileNet`` hands an fp32 input with a dense decoder to the engine only under ``'high'`` or
 ``'medium'``: split TF32 stays within the fp32 bound of 1e-3 where cuDNN's plain TF32 convs do not.
 
-One plan per (device, H, W, dtype) is live at a time.  A batch no larger than its capacity runs on it (the C-ABI builds
-the steps for that batch size once, over the plan's buffers and weights; ``fd_forward_batch``); a larger batch replaces it
-with a plan sized for that batch.  So an evaluation with a short last batch, or a serving loop that sees many batch sizes,
-holds one set of activation buffers and packed weights instead of one per batch size.
+One plan per (device, dtype) is live at a time.  A request [n,3,h,w] whose pixels n*h*w fit the plan's capacity (the
+n*h*w it was built for) runs on it, whatever its batch size and resolution (the C-ABI builds the steps for that shape once,
+over the plan's buffers and weights; ``fd_forward_shape``).  A larger request replaces it with a plan built for the
+request's own shape, whose capacity covers everything the old one served.  So an evaluation with a short last batch, or a
+serving loop that sees many batch sizes and resolutions (224x224 and 480x640, say), holds one set of activation buffers
+and packed weights instead of one per shape.
 """
 import torch
 
@@ -26,7 +28,7 @@ _SUPPORTED = (torch.float32, torch.float16, torch.bfloat16)
 class SkipAddEngine:
     def __init__(self, module):
         self.module = module
-        self.plans = {}          # (device index, h, w, dtype) -> Plan (its n: the largest batch seen since the last refresh)
+        self.plans = {}          # (device index, dtype) -> Plan (built for the largest n*h*w seen since the last refresh)
         self.signature = None
         self.options = {}
 
@@ -67,8 +69,9 @@ class SkipAddEngine:
 
     # -- forward ---------------------------------------------------------------------------------
     def plan_for(self, x, exact=False):
-        """The plan that runs ``x``: the live plan of its (device, H, W, dtype) if its capacity holds ``x.shape[0]`` images
-        (``exact``: equals it, as the host pipeline needs), else a new plan sized for ``x`` that replaces it."""
+        """The plan that runs ``x``: the live plan of its (device, dtype) if the pixels of ``x`` (n*h*w) fit its capacity
+        (``exact``: its own (n, h, w) equals that of ``x``, as the host pipeline needs), else a new plan built for the shape
+        of ``x`` that replaces it."""
         m = self.module
         if m.training:
             raise RuntimeError("fastdepth_b200 is inference-only: call model.eval() first "
@@ -91,9 +94,9 @@ class SkipAddEngine:
         if sig != self.signature:
             self.refresh()
             self.signature = sig
-        key = (x.device.index, h, w, x.dtype)
+        key = (x.device.index, x.dtype)
         p = self.plans.get(key)
-        if p is not None and (n > p.n or (exact and n != p.n)):
+        if p is not None and (n * h * w > p.n * p.h * p.w or (exact and (n, h, w) != (p.n, p.h, p.w))):
             del self.plans[key]       # freed with its last reference (a pending host-pipeline ticket holds one)
             p = None
         if p is None:

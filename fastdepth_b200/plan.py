@@ -203,8 +203,8 @@ def _fp(a):
 
 
 class Plan:
-    """Owns one ``fd_plan`` (H,W,dtype,device and a batch capacity N; ``forward`` runs any batch up to N).  Thin: every
-    method is one C-ABI call."""
+    """Owns one ``fd_plan`` built for (N, H, W, dtype, device); ``forward`` runs any (n, h, w) with h, w multiples of 32 and
+    n*h*w <= N*H*W.  Thin: every method is one C-ABI call."""
 
     def __init__(self, descs, weights, names, n, h, w, dtype, device_index):
         self.lib = _lib.load()
@@ -237,13 +237,11 @@ class Plan:
         return v.value
 
     def forward(self, x, y, stream_ptr, n=None):
-        """Forward of the first ``n`` images (default ``x.shape[0]``), 1 <= n <= the plan's n; a smaller batch runs on
-        the plan's buffers through ``fd_forward_batch``."""
+        """Forward of the first ``n`` images (default ``x.shape[0]``) of ``x`` at its own resolution, through
+        ``fd_forward_shape``: any shape whose pixels n*h*w fit the plan's n*h*w runs on the plan's buffers."""
         n = x.shape[0] if n is None else int(n)
-        if n == self.n:
-            _lib.check(self.lib.fd_forward(self.handle, x.data_ptr(), y.data_ptr(), stream_ptr))
-        else:
-            _lib.check(self.lib.fd_forward_batch(self.handle, n, x.data_ptr(), y.data_ptr(), stream_ptr))
+        _lib.check(self.lib.fd_forward_shape(self.handle, n, x.shape[2], x.shape[3], x.data_ptr(), y.data_ptr(),
+                                             stream_ptr))
 
     def forward_host(self, x_host, y_host, stream_ptr):
         _lib.check(self.lib.fd_forward_host(self.handle, x_host.data_ptr(), y_host.data_ptr(), stream_ptr))

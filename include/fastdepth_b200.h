@@ -160,13 +160,21 @@ int fd_plan_get_option(fd_plan* plan, const char* name, int* value);
  * Replaces: pred = model(input)  (reference main.py:74-75 -> models.py:706-732). */
 int fd_forward(fd_plan* plan, const void* x_dev, void* y_dev, void* stream);
 
-/* The same forward over the first n images, 1 <= n <= the plan's N: x_dev is [n,3,H,W] and y_dev [n,1,H,W], and nothing
- * is read or written past image n (FD_ERR_INVALID for any other n).  The result equals that of a plan built for n, bit for
- * bit.  The plan builds the steps for n on first use (planner choices, grids, tensor maps) over its own activation buffers,
- * packed weights and split weights; it keeps up to 8 such step sets, least recently used first out (the set of its own N is
- * always kept), and captures graphs per (x_dev, y_dev, n).  fd_forward(plan, ...) is fd_forward_batch(plan, N, ...).
- * fd_forward_host and fd_pipeline_* always run N images. */
+/* The same forward over the first n images, 1 <= n <= the plan's N, at the plan's own H x W: fd_forward_shape(plan, n, H,
+ * W, ...).  x_dev is [n,3,H,W] and y_dev [n,1,H,W]. */
 int fd_forward_batch(fd_plan* plan, int n, const void* x_dev, void* y_dev, void* stream);
+
+/* The forward of n images at any resolution h x w that fits the plan's pixel capacity: x_dev is [n,3,h,w] and y_dev
+ * [n,1,h,w], contiguous, plan dtype.  Accepted: n >= 1, h and w positive multiples of 32, n*h*w <= N*H*W (every stage
+ * buffer of the plan is dense NHWC of N*(H/s)*(W/s)*C elements, so the request fits in its front).  Anything else fails
+ * with FD_ERR_INVALID; for a request that does not fit, the message names the capacity in pixels and the plan's (N, H, W).
+ * Nothing is read or written past n*h*w elements of x_dev (times 3) or y_dev.  The result equals that of a plan built for
+ * (n, h, w), bit for bit.  The plan builds the steps for (n, h, w) on first use (every stage's geometry, planner choices,
+ * grids, tensor maps, whether a run of blocks takes the chain kernel) over its own activation buffers, packed weights and
+ * split weights; it keeps up to 8 such step sets, least recently used first out (the set of its own (N, H, W) is always
+ * kept), and captures graphs per (x_dev, y_dev, n, h, w).  fd_forward(plan, ...) is fd_forward_shape(plan, N, H, W, ...).
+ * fd_forward_host and fd_pipeline_* always run N images at H x W. */
+int fd_forward_shape(fd_plan* plan, int n, int h, int w, const void* x_dev, void* y_dev, void* stream);
 
 /* Same, end to end from HOST buffers: H2D copy of x, forward, D2H copy of y, then waits for
  * the stream.  (reference main.py:68 input.cuda() ... main.py:85-98 pred.cpu()) */
@@ -189,10 +197,10 @@ int fd_stage_buffer(fd_plan* plan, int stage, int which, void** dev_ptr,
 
 /* Bookkeeping used by bench.py.  A "step" is one kernel launch of fd_forward under the current
  * options (a DWPW stage is one fused step on path 1, or two under "unfuse"; a dw + a pw step on path 0); the step functions, fd_plan_time_steps,
- * fd_plan_trace_stage and fd_stage_buffer describe the steps of the plan's own N.  The workspace bytes include, once the
- * steps are built, the device memory they hold: with "tf32x3", the split weights [2][c_out][k*k][c_in] fp32 of every
- * split-TF32 step (once, shared by every batch size), and the packed parameter copies of every step set fd_forward_batch
- * built for a batch size below N. */
+ * fd_plan_trace_stage and fd_stage_buffer describe the steps of the plan's own (N, H, W).  The workspace bytes include, once
+ * the steps are built, the device memory they hold: with "tf32x3", the split weights [2][c_out][k*k][c_in] fp32 of every
+ * split-TF32 step (once, shared by every shape), and the packed parameter copies of every step set fd_forward_shape
+ * built for a shape other than (N, H, W). */
 int fd_plan_launches_per_forward(fd_plan* plan, int* n_launches);
 int fd_plan_workspace_bytes(fd_plan* plan, size_t* bytes);
 int fd_plan_step_count(fd_plan* plan, int* n_steps);
