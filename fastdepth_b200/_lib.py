@@ -54,6 +54,8 @@ SIGNATURES = {
                                            _c_int_p, _c_int_p]),
     'fd_debug_block_plan': (ctypes.c_int, [ctypes.c_int] * 8 + [_c_int_p, ctypes.c_int]),
     'fd_debug_conv_plan': (ctypes.c_int, [ctypes.c_int] * 7 + [_c_int_p, ctypes.c_int]),
+    'fd_debug_front_plan': (ctypes.c_int, [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                           _c_int_p, ctypes.c_int]),
     'fd_debug_convt_plan': (ctypes.c_int, [ctypes.c_int] * 8 + [_c_int_p, ctypes.c_int]),
     'fd_debug_pw_tf32x3_plan': (ctypes.c_int, [ctypes.c_int] * 7 + [_c_int_p, ctypes.c_int]),
     'fd_debug_pw_plan': (ctypes.c_int, [ctypes.c_int] * 7 + [_c_int_p, ctypes.c_int]),

@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libfastdepth_b200.so')
-SOURCES = ('fd_api.cu', 'fd_kernels_simt.cu', 'fd_block_tc.cu', 'fd_chain_tc.cu', 'fd_stem_tc.cu', 'fd_conv_tc.cu',
+SOURCES = ('fd_api.cu', 'fd_kernels_simt.cu', 'fd_block_tc.cu', 'fd_chain_tc.cu', 'fd_stem_tc.cu', 'fd_front_tc.cu', 'fd_conv_tc.cu',
            'fd_metrics.cu')
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC']

@@ -66,6 +66,18 @@ int stem_tc_prepare(int dtype, const StageGeom& g, const float* w27_dev, const f
 int stem_tc_launch(StemTcPlan* sp, const void* x, cudaStream_t st);
 void stem_tc_destroy(StemTcPlan* sp);
 const char* stem_tc_name(StemTcPlan* sp);
+// stem + conv1 + conv2 as one kernel (fd_front_tc.cu)
+struct FrontTcPlan;
+bool front_tc_shape_ok(int dtype, const StageGeom& g0, const StageGeom& g1, const StageGeom& g2);
+int front_tc_items(int n, int h, int w);
+void front_tc_layout(int* out);
+int front_tc_prepare(int dtype, const StageGeom& g0, const StageGeom& g1, const StageGeom& g2, const float* w27,
+                     const float* sc0, const float* bi0, const BlockArgs& a1, const BlockArgs& a2, void* out0,
+                     const TcLaunchOpts& opts, FrontTcPlan** res);
+int front_tc_launch(FrontTcPlan* fp, const void* x, cudaStream_t st);
+void front_tc_destroy(FrontTcPlan* fp);
+const char* front_tc_name(FrontTcPlan* fp);
+size_t front_tc_param_bytes(FrontTcPlan* fp);
 // dense kxk conv on wgmma (fd_conv_tc.cu)
 struct ConvTcPlan;
 bool conv_tc_supported(int dtype, const StageGeom& g, int kind);
@@ -127,8 +139,9 @@ struct StageRun {
     StemTcPlan* stc = nullptr;
     ConvTcPlan* ctc = nullptr;
     ChainTcPlan* chain = nullptr;        // set on the FIRST stage of a run executed by the chain kernel
-    int chained = 0;                     // 1: this stage runs inside a chain kernel (its own output buffer is only written if it is
-                                         //    the run's last stage)
+    FrontTcPlan* front = nullptr;        // set on the stem when stages 0..2 run as one front_tc_kernel step
+    int chained = 0;                     // 1: this stage runs inside a kernel launched at an earlier stage: a chain kernel (its own
+                                         //    output buffer is only written if it is the run's last stage) or the front kernel
     void* out_eff = nullptr;             // buffer the stage really writes (== a skip source when accumulating in place)
 };
 
@@ -172,6 +185,7 @@ struct fd_plan {
     int opt_cluster = 1;
     int opt_tf32x3 = 0;
     int opt_unfuse = 1;
+    int opt_front = 1;
     size_t workspace_bytes = 0;
     size_t split_bytes = 0;              // device memory of the stages' split weights (tf32x3), freed with the step sets
     // fd_pipeline_*: host batches flow H2D -> forward -> D2H through kPipeSlots device slots on three streams
@@ -229,6 +243,7 @@ static void destroy_set(StepSet* ss) {
         if (r.stc) stem_tc_destroy(r.stc);
         if (r.ctc) conv_tc_destroy(r.ctc);
         if (r.chain) chain_tc_destroy(r.chain);
+        if (r.front) front_tc_destroy(r.front);
     }
     delete ss;
 }
@@ -349,6 +364,17 @@ static int walk_stages(const fd_stage_desc* stages, int n_stages, int n, int h, 
     return FD_OK;
 }
 
+// The front route (plan option "front"): the stem and the two DWPW stages after it run as one front_tc_kernel step when the
+// three have the stock MobileNet shapes (front_tc_shape_ok), neither block takes a skip or upsamples, and no stage
+// concatenates onto one of their outputs (a channel slice of a wider buffer).  A 16-bit plan on path 1 only.
+static bool front_route_ok(const fd_stage_desc* D, int ns, int dtype, const std::vector<StageShape>& S) {
+    if (ns < 4 || D[0].kind != FD_STAGE_STEM || D[1].kind != FD_STAGE_DWPW || D[2].kind != FD_STAGE_DWPW) return false;
+    if (D[1].skip_src >= 0 || D[2].skip_src >= 0) return false;
+    for (int j = 3; j < ns; ++j)
+        if (D[j].skip_src >= 0 && D[j].skip_src <= 2 && D[j].skip_mode) return false;
+    return front_tc_shape_ok(dtype, S[0].g, S[1].g, S[2].g);
+}
+
 // Build the steps of a forward of n images at h x w into `ss`: every stage's geometry at that shape, over the front of the
 // plan's buffers.  Every decision that depends on the geometry (the chain kernel, the two-step route, the planners) is
 // taken from the set's own geometry, as a plan built for (n, h, w) takes it.
@@ -396,7 +422,39 @@ static int build_steps(fd_plan* p, int n, int h, int w, StepSet* ss) {
                            29.0 * sg.c_out * 4;
             Stage* sp = &s;
             const int dtype = p->dtype;
-            if (p->opt_path == 1 && stem_tc_supported(dtype, sg)) {
+            if (p->opt_path == 1 && p->opt_front && front_route_ok(D.data(), ns, dtype, S) && stem_tc_supported(dtype, sg)) {
+                // stem + conv1 + conv2 as one step that writes all three buffers and reads only x; reported under stage 2,
+                // the last buffer it writes, as a chain run is
+                BlockArgs a[2]{};
+                StageGeom g[3] = {sg, G[1], G[2]};
+                for (int k = 1; k <= 2; ++k) {
+                    Stage& t = p->stages[k];
+                    g[k].in_pitch = p->stages[k - 1].out_pitch; g[k].out_pitch = t.out_pitch;
+                    BlockArgs& b = a[k - 1];
+                    b.g = g[k]; b.out = t.out;
+                    b.dw_w = t.dw_w; b.dw_scale = t.dw_scale; b.dw_bias = t.dw_bias;
+                    b.pw_w = t.pw_w; b.pw_scale = t.pw_scale; b.pw_bias = t.pw_bias;
+                }
+                int rc = front_tc_prepare(dtype, g[0], g[1], g[2], s.pw_w_f32, s.pw_scale, s.pw_bias, a[0], a[1], s.out, lopts, &r.front);
+                if (rc != FD_OK) return rc;
+                ss->bytes += front_tc_param_bytes(r.front);
+                st.stage = 2;
+                st.name = front_tc_name(r.front);
+                st.dw_macs = 0.0;
+                double wb = 29.0 * sg.c_out * 4, out_px_bytes = (double)sg.n * sg.h_out * sg.w_out * sg.c_out;
+                for (int k = 1; k <= 2; ++k) {
+                    const double px = (double)g[k].n * g[k].h_out * g[k].w_out;
+                    st.dw_macs += px * g[k].c_in * 9.0;
+                    st.macs += px * g[k].c_in * 9.0 + px * g[k].c_in * g[k].c_out;
+                    wb += (double)g[k].c_in * 9 * 4 + 2.0 * g[k].c_in * 4 + (double)g[k].c_in * g[k].c_out * es + 2.0 * g[k].c_out * 4;
+                    out_px_bytes += px * g[k].c_out;
+                    R[k].chained = 1;
+                    R[k].out_eff = p->stages[k].out;
+                }
+                st.alg_bytes = ((double)sg.n * 3 * sg.h_in * sg.w_in + out_px_bytes) * es + wb;
+                FrontTcPlan* fp = r.front;
+                st.run = [fp](cudaStream_t stream, const void* x, void*) { return front_tc_launch(fp, x, stream); };
+            } else if (p->opt_path == 1 && stem_tc_supported(dtype, sg)) {
                 int rc = stem_tc_prepare(dtype, sg, s.pw_w_f32, s.pw_scale, s.pw_bias, s.out, lopts, &r.stc);
                 if (rc != FD_OK) return rc;
                 ss->bytes += stem_tc_param_bytes(r.stc);
@@ -832,6 +890,7 @@ static int* option_slot(fd_plan* p, const char* name) {
     if (!strcmp(name, "cluster")) return &p->opt_cluster;
     if (!strcmp(name, "tf32x3")) return &p->opt_tf32x3;
     if (!strcmp(name, "unfuse")) return &p->opt_unfuse;
+    if (!strcmp(name, "front")) return &p->opt_front;
     return nullptr;
 }
 
@@ -1192,6 +1251,19 @@ int fd_debug_block_plan(int ksize, int stride, int h_out, int w_out, int n, int 
     const int v[16] = {q.ok, q.splits, q.n_cta, q.items, q.kblocks, q.s_in, q.s_a, q.s_b, q.bn, q.nb, q.b_resident, q.n_stg,
                        q.smem_bytes, q.in_stage_stride, q.cs, q.dw_teams};
     for (int i = 0; i < 16; ++i) out[i] = v[i];
+    return FD_OK;
+}
+
+int fd_debug_front_plan(const fd_stage_desc* stages, int n_stages, int dtype, int n, int h, int w, int* out, int cap) {
+    if (!out || cap < 8) return fail(FD_ERR_INVALID, "need an int[8] output");
+    if (!stages || n_stages < 1) return fail(FD_ERR_INVALID, "no stages");
+    std::vector<StageShape> S;
+    const int rc = walk_stages(stages, n_stages, n, h, w, S);
+    if (rc != FD_OK) return rc;
+    const bool ok = front_route_ok(stages, n_stages, dtype, S);
+    out[0] = ok ? 1 : 0;
+    out[1] = ok ? front_tc_items(n, h, w) : 0;
+    front_tc_layout(out + 2);
     return FD_OK;
 }
 

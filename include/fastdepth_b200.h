@@ -146,6 +146,12 @@ int fd_plan_set_stage_weights(fd_plan* plan, int stage,
  *                stage inside a chain, a skip only with "tma_epilogue" and "inplace_skip").  A stage whose block-kernel
  *                plan is pinned by FD_TC_MAX_NCTA, FD_TC_CLUSTER >= 2, FD_TC_WMC or FD_TC_DW_TEAMS stays fused.
  *                fd_stage_buffer(which = 1) returns the intermediate of a two-step stage.  [default 1]
+ *   "front"      1 = in a 16-bit plan on path 1 the stem and the two DWPW stages after it run as ONE kernel
+ *                (front_tc_kernel) when they have the stock MobileNet shapes: stem 3 -> 32 stride 2 with ReLU6, 3x3
+ *                blocks 32 -> 64 stride 1 and 64 -> 128 stride 2 with one act, no skip, no concatenation onto their
+ *                outputs.  An item is an 8x8 tile of conv2's output; the conv0 and conv1 pixels it needs are computed in
+ *                shared memory and each stage's own part is written to its buffer, so conv0 and conv1 are never read back.
+ *                The result is the three kernels', bit for bit.  0 = three steps.  [default 1]
  *   "wait_sleep_ns" > 0: latency-tolerant roles of the fused block kernel (the TMA producer waiting for a
  *                free stage) sleep this many ns between barrier
  *                probes instead of spinning (the spinning waiters do not
@@ -254,6 +260,12 @@ int fd_debug_pw_tf32x3_plan(int h_out, int w_out, int n, int c_in, int c_out, in
  * them.  out[0..13] as in fd_debug_conv_plan (kblocks of 64 channels); out[14] = bytes of one operand stage (16 KB of A +
  * bn x 128 B of B), out[15] = 0.  cap must be at least 16. */
 int fd_debug_pw_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsample, int n_sms, int* out, int cap);
+
+/* Debug (host only, needs no GPU): whether a 16-bit plan on path 1 of these stages at n x h x w runs its stem and the two
+ * blocks after it as one front_tc_kernel step ("front"), and that kernel's budget.  out[0] = 1 when it does, out[1] = its
+ * items (8x8 tiles of conv2's map, 0 when it does not), out[2] = dynamic shared memory per CTA in bytes, out[3] = CTAs per
+ * SM, out[4] = threads per CTA, out[5..7] = bytes of its weight + parameter, A-operand and tile regions.  cap >= 8. */
+int fd_debug_front_plan(const fd_stage_desc* stages, int n_stages, int dtype, int n, int h, int w, int* out, int cap);
 
 int fd_debug_convt_plan(int kind, int ksize, int h_in, int w_in, int n, int c_in, int c_out, int n_sms, int* out, int cap);
 
