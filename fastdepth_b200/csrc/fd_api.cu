@@ -70,7 +70,7 @@ const char* stem_tc_name(StemTcPlan* sp);
 struct FrontTcPlan;
 bool front_tc_shape_ok(int dtype, const StageGeom& g0, const StageGeom& g1, const StageGeom& g2);
 int front_tc_items(int n, int h, int w);
-void front_tc_layout(int* out);
+void front_tc_layout(int cin, int* out);
 int front_tc_prepare(int dtype, const StageGeom& g0, const StageGeom& g1, const StageGeom& g2, const float* w27,
                      const float* sc0, const float* bi0, const BlockArgs& a1, const BlockArgs& a2, void* out0,
                      const TcLaunchOpts& opts, FrontTcPlan** res);
@@ -300,7 +300,13 @@ static int upload_as_dtype(int dtype, const float* host, size_t count, void* dev
 static int walk_stages(const fd_stage_desc* stages, int n_stages, int n, int h, int w, std::vector<StageShape>& out) {
     out.assign(n_stages, StageShape());
     std::vector<int> concat_src(n_stages, -1);         // >= 0: the stage's output is a channel slice of that stage's buffer
-    int ch = 3, hh = h, ww = w;
+    // the stem reads c_in planes of x: 1..7 (RGB 3, depth only 1, RGB-D 4; K = 9 c_in fits one 64-element row of the
+    // tensor-core stem).  8 or more would need a second K block per im2col row
+    const int c_x = stages[0].c_in;
+    if (stages[0].kind == FD_STAGE_STEM && c_x <= 0) return fail(FD_ERR_INVALID, "stem c_in must be positive");
+    if (stages[0].kind == FD_STAGE_STEM && c_x > 7)
+        return fail(FD_ERR_UNSUPPORTED, "stem c_in " + std::to_string(c_x) + " is not supported: the stem takes 1..7 input channels");
+    int ch = c_x, hh = h, ww = w;
     for (int i = 0; i < n_stages; ++i) {
         const fd_stage_desc& d = stages[i];
         StageShape& s = out[i];
@@ -313,8 +319,8 @@ static int walk_stages(const fd_stage_desc* stages, int n_stages, int n, int h, 
         s.g.n = n; s.g.h_in = hh; s.g.w_in = ww; s.g.c_in = d.c_in; s.g.c_out = d.c_out;
         s.g.ksize = d.ksize; s.g.stride = d.stride; s.g.act = d.act; s.g.upsample = d.upsample ? 1 : 0;
         if (d.kind == FD_STAGE_STEM) {
-            if (d.ksize != 3 || d.c_in != 3 || d.c_out % 8 || d.stride < 1 || d.stride > 2 || d.upsample || d.skip_src >= 0)
-                return fail(FD_ERR_INVALID, "stem must be 3x3, c_in 3, c_out % 8 == 0, stride 1|2");
+            if (d.ksize != 3 || d.c_out % 8 || d.stride < 1 || d.stride > 2 || d.upsample || d.skip_src >= 0)
+                return fail(FD_ERR_INVALID, "stem must be 3x3, c_out % 8 == 0, stride 1|2");
             s.g.h_out = (hh + 2 - 3) / d.stride + 1; s.g.w_out = (ww + 2 - 3) / d.stride + 1;
         } else if (d.kind == FD_STAGE_DWPW) {
             if ((d.ksize != 3 && d.ksize != 5) || d.stride < 1 || d.stride > 2 || d.c_in % 8 || d.c_out % 8 || d.c_out <= 0)
@@ -416,10 +422,10 @@ static int build_steps(fd_plan* p, int n, int h, int w, StepSet* ss) {
         if (s.d.kind == FD_STAGE_STEM) {
             Step st;
             st.stage = i;
-            st.name = "stem_kernel";
-            st.macs = (double)sg.n * sg.h_out * sg.w_out * sg.c_out * 27.0;
-            st.alg_bytes = ((double)sg.n * 3 * sg.h_in * sg.w_in + (double)sg.n * sg.h_out * sg.w_out * sg.c_out) * es +
-                           29.0 * sg.c_out * 4;
+            st.name = sg.c_in == 3 ? "stem_kernel" : "stem_kernel<cin" + std::to_string(sg.c_in) + ">";
+            st.macs = (double)sg.n * sg.h_out * sg.w_out * sg.c_out * 9.0 * sg.c_in;
+            st.alg_bytes = ((double)sg.n * sg.c_in * sg.h_in * sg.w_in + (double)sg.n * sg.h_out * sg.w_out * sg.c_out) * es +
+                           (9.0 * sg.c_in + 2.0) * sg.c_out * 4;
             Stage* sp = &s;
             const int dtype = p->dtype;
             if (p->opt_path == 1 && p->opt_front && front_route_ok(D.data(), ns, dtype, S) && stem_tc_supported(dtype, sg)) {
@@ -441,7 +447,7 @@ static int build_steps(fd_plan* p, int n, int h, int w, StepSet* ss) {
                 st.stage = 2;
                 st.name = front_tc_name(r.front);
                 st.dw_macs = 0.0;
-                double wb = 29.0 * sg.c_out * 4, out_px_bytes = (double)sg.n * sg.h_out * sg.w_out * sg.c_out;
+                double wb = (9.0 * sg.c_in + 2.0) * sg.c_out * 4, out_px_bytes = (double)sg.n * sg.h_out * sg.w_out * sg.c_out;
                 for (int k = 1; k <= 2; ++k) {
                     const double px = (double)g[k].n * g[k].h_out * g[k].w_out;
                     st.dw_macs += px * g[k].c_in * 9.0;
@@ -451,7 +457,7 @@ static int build_steps(fd_plan* p, int n, int h, int w, StepSet* ss) {
                     R[k].chained = 1;
                     R[k].out_eff = p->stages[k].out;
                 }
-                st.alg_bytes = ((double)sg.n * 3 * sg.h_in * sg.w_in + out_px_bytes) * es + wb;
+                st.alg_bytes = ((double)sg.n * sg.c_in * sg.h_in * sg.w_in + out_px_bytes) * es + wb;
                 FrontTcPlan* fp = r.front;
                 st.run = [fp](cudaStream_t stream, const void* x, void*) { return front_tc_launch(fp, x, stream); };
             } else if (p->opt_path == 1 && stem_tc_supported(dtype, sg)) {
@@ -796,7 +802,7 @@ int fd_plan_create(const fd_stage_desc* stages, int n_stages, int n, int h, int 
         } else if (is_conv(d.kind)) {
             if ((rc = dev_alloc(p, &s.pw_w, (size_t)d.ksize * d.ksize * d.c_in * d.c_out * es))) break;
         } else if (d.kind == FD_STAGE_STEM) {
-            if ((rc = dev_alloc(p, (void**)&s.pw_w_f32, (size_t)27 * d.c_out * 4))) break;
+            if ((rc = dev_alloc(p, (void**)&s.pw_w_f32, (size_t)9 * d.c_in * d.c_out * 4))) break;
         } else {
             if ((rc = dev_alloc(p, (void**)&s.pw_w_f32, (size_t)d.c_in * 4))) break;
         }
@@ -861,9 +867,10 @@ int fd_plan_set_stage_weights(fd_plan* p, int stage, const float* dw_w, const fl
         int rc = upload_as_dtype(p->dtype, t.data(), t.size(), s.pw_w);
         if (rc) return rc;
     } else if (d.kind == FD_STAGE_STEM) {
-        std::vector<float> t((size_t)27 * d.c_out);            // [co][ci][ky][kx] -> [(ci,ky,kx)][co]
+        const int nk = 9 * d.c_in;
+        std::vector<float> t((size_t)nk * d.c_out);            // [co][ci][ky][kx] -> [(ci,ky,kx)][co]
         for (int co = 0; co < d.c_out; ++co)
-            for (int j = 0; j < 27; ++j) t[(size_t)j * d.c_out + co] = pw_w[(size_t)co * 27 + j];
+            for (int j = 0; j < nk; ++j) t[(size_t)j * d.c_out + co] = pw_w[(size_t)co * nk + j];
         FD_CUDA_OK(cudaMemcpy(s.pw_w_f32, t.data(), t.size() * 4, cudaMemcpyHostToDevice));
     } else {
         FD_CUDA_OK(cudaMemcpy(s.pw_w_f32, pw_w, (size_t)d.c_in * 4, cudaMemcpyHostToDevice));
@@ -1042,7 +1049,7 @@ int fd_forward_host(fd_plan* p, const void* x_host, void* y_host, void* stream) 
     if (!p || !x_host || !y_host) return fail(FD_ERR_INVALID, "NULL argument");
     DeviceGuard guard(p->device);
     const size_t es = dtype_size(p->dtype);
-    const size_t xb = (size_t)p->n * 3 * p->h * p->w * es, yb = (size_t)p->n * p->h * p->w * es;
+    const size_t xb = (size_t)p->n * p->stages[0].d.c_in * p->h * p->w * es, yb = (size_t)p->n * p->h * p->w * es;
     if (!p->stage_x) {
         int rc = dev_alloc(p, &p->stage_x, xb);
         if (rc) return rc;
@@ -1063,7 +1070,7 @@ int fd_pipeline_submit(fd_plan* p, const void* x_host, void* y_host, unsigned lo
     if (!p || !x_host || !y_host || !ticket) return fail(FD_ERR_INVALID, "NULL argument");
     DeviceGuard guard(p->device);
     const size_t es = dtype_size(p->dtype);
-    const size_t xb = (size_t)p->n * 3 * p->h * p->w * es, yb = (size_t)p->n * p->h * p->w * es;
+    const size_t xb = (size_t)p->n * p->stages[0].d.c_in * p->h * p->w * es, yb = (size_t)p->n * p->h * p->w * es;
     if (!p->pipe_h2d) {
         FD_CUDA_OK(cudaStreamCreateWithFlags(&p->pipe_h2d, cudaStreamNonBlocking));
         FD_CUDA_OK(cudaStreamCreateWithFlags(&p->pipe_run, cudaStreamNonBlocking));
@@ -1263,7 +1270,7 @@ int fd_debug_front_plan(const fd_stage_desc* stages, int n_stages, int dtype, in
     const bool ok = front_route_ok(stages, n_stages, dtype, S);
     out[0] = ok ? 1 : 0;
     out[1] = ok ? front_tc_items(n, h, w) : 0;
-    front_tc_layout(out + 2);
+    front_tc_layout(S[0].g.c_in, out + 2);
     return FD_OK;
 }
 

@@ -1,11 +1,12 @@
-// The front of the encoder as ONE kernel: stem (3x3 s2, 3 -> C0) -> DWPW 3x3 s1 (C0 -> C1) -> DWPW 3x3 s2 (C1 -> C2).
+// The front of the encoder as ONE kernel: stem (3x3 s2, c_in -> C0) -> DWPW 3x3 s1 (C0 -> C1) -> DWPW 3x3 s2 (C1 -> C2),
+// for c_in = 1..4 input channels (RGB: 3, depth only: 1, RGB-D: 4).
 //
 // The three separate steps move 379 MB at b64 224x224, and 154 MB of that is conv1 reading back the map the stem has just
 // written and conv2 reading back conv1's.  Here an item is one 8x8 tile of conv2's output; the CTA computes the conv0 and
 // conv1 pixels that tile needs (with their 3x3 halos) in shared memory, writes the part of each it owns to its stage buffer
 // and never reads either back from HBM:
 //
-//   x box    3 planes x 39 rows x 48 cols (TMA, OOB zero fill = the stem's padding), 16 bytes left of the needed columns
+//   x box    c_in planes x 39 rows x 48 cols (TMA, OOB zero fill = the stem's padding), 16 bytes left of the needed columns
 //   T0       19 x 19 conv0 pixels x C0: rows / cols 2..17 are this item's part of the conv0 buffer; pixels outside the map are 0
 //   T1       17 x 17 conv1 pixels x C1: rows / cols 1..16 -> the conv1 buffer; pixels outside the map are 0
 //   out      8 x 8 conv2 pixels x C2 -> the conv2 buffer
@@ -16,9 +17,11 @@
 // a whole output row of one channel pair and widens each input word once for every output that uses it.  Two CTAs share
 // an SM (front_tc_smem_bytes), so one CTA's phases overlap the other's.  The x box shares the A region with the stem chunk
 // and conv2's operand but not with conv1's, so the next item's box loads from the end of conv1's GEMM through all of conv2.
+// Three planes fit in conv1's A region beside the stem chunk; a fourth runs 2688 bytes past it, so at c_in = 4 the tiles
+// region moves up by that much and the CTA still fits twice per SM.  Five or more planes do not fit twice (front_tc_layout).
 //
 // Same bits as stem_tc_kernel + block_tc_kernel (HALFK for conv1): the stem's taps sit in the same K positions and run as
-// two k16 steps from a zero accumulator; a depthwise output is one fp32 FMA per tap with ky outer and kx inner from +0 over
+// ceil(9 c_in / 16) k16 steps from a zero accumulator (two at c_in = 3); a depthwise output is one fp32 FMA per tap with ky outer and kx inner from +0 over
 // 16-bit taps widened to fp32 (the zero pixels outside the map add +0 or -0 to an accumulator that starts at +0, which
 // leaves it unchanged), then ffma2_abc BN and pack_act; conv1's pointwise GEMM issues K = 64 against zero channels
 // 32..63 as the HALFK block kernel does; every epilogue is ffma2_abc + pack_act on the same fragment.
@@ -35,20 +38,25 @@ constexpr int FR_THREADS = 256;
 constexpr int FR_C0 = 32, FR_C1 = 64, FR_C2 = 128;
 constexpr int FR_T0 = 19, FR_T1 = 17, FR_T2 = 8;            // tile edges of conv0, conv1, conv2
 constexpr int FR_XH = 39, FR_XW = 48;                       // x box: rows 4*oy2 - 5 .., columns 4*ox2 - 8 ..
-constexpr int FR_X_BYTES = 3 * FR_XH * FR_XW * 2;           // 11232
+constexpr int FR_MAX_CIN = 4;                               // planes of the x box for which two CTAs fit on an SM
 constexpr int FR_A0_ROWS = 192;                             // stem A operand: two chunks of three m64 blocks (361 rows)
 // shared-memory layout (offsets from the 1 KB-aligned base); SWIZZLE_128B operands first
 constexpr uint32_t FR_W0 = 0, FR_W1 = FR_W0 + FR_C0 * 128, FR_W2 = FR_W1 + FR_C1 * 128;
 constexpr uint32_t FR_R1 = FR_W2 + FR_C2 * 128;             // A operands: stem chunk (24 KB), conv1 (320 rows, 40 KB), conv2 (8 KB)
 constexpr uint32_t FR_X = FR_R1 + 28672;                    // x box: beside the stem chunk and conv2's A, inside conv1's A
-constexpr uint32_t FR_R2 = FR_R1 + 320 * 128;               // T0, then T1, then conv2's output staging
-constexpr uint32_t FR_PRM = FR_R2 + 37120;                  // after T1 (289 x 128 B)
+// x box bytes (11232 at c_in = 3) and how far they run past conv1's A region (rounded to 128 B; 0 for c_in <= 3)
+__host__ __device__ constexpr uint32_t fr_x_bytes(int cin) { return (uint32_t)cin * FR_XH * FR_XW * 2; }
+__host__ __device__ constexpr uint32_t fr_x_over(int cin) {
+    return FR_X + fr_x_bytes(cin) > FR_R1 + 320 * 128 ? (FR_X + fr_x_bytes(cin) - (FR_R1 + 320 * 128) + 127) / 128 * 128 : 0;
+}
+__host__ __device__ constexpr uint32_t fr_r2(int cin) { return FR_R1 + 320 * 128 + fr_x_over(cin); }   // T0, then T1, then conv2's output staging
+__host__ __device__ constexpr uint32_t fr_prm(int cin) { return fr_r2(cin) + 37120; }                  // after T1 (289 x 128 B)
 // parameter block (global blob after the weights, copied verbatim): dw taps [9][C] 16-bit, dw scale [C] + bias [C] fp32,
 // pointwise (scale, scale, bias, bias) per channel pair
 constexpr uint32_t FR_P_TAP1 = 0, FR_P_SB1 = FR_P_TAP1 + 9 * FR_C0 * 2, FR_P_TAP2 = FR_P_SB1 + 2 * FR_C0 * 4;
 constexpr uint32_t FR_P_SB2 = FR_P_TAP2 + 9 * FR_C1 * 2, FR_P_AFF0 = FR_P_SB2 + 2 * FR_C1 * 4;
 constexpr uint32_t FR_P_AFF1 = FR_P_AFF0 + FR_C0 * 8, FR_P_AFF2 = FR_P_AFF1 + FR_C1 * 8, FR_P_BYTES = FR_P_AFF2 + FR_C2 * 8;
-constexpr uint32_t FR_BAR = FR_PRM + FR_P_BYTES;
+__host__ __device__ constexpr uint32_t fr_bar(int cin) { return fr_prm(cin) + FR_P_BYTES; }
 constexpr uint32_t FR_W_BYTES = (FR_C0 + FR_C1 + FR_C2) * 128;    // weights in the blob: [224 rows][64] 16-bit, K-major
 
 struct FrontParams {
@@ -61,19 +69,29 @@ struct FrontParams {
     const uint4* blob;                 // weights [224][64] 16-bit, then the parameter block
 };
 
-size_t front_tc_smem_bytes() { return (size_t)FR_BAR + 8 + 1024; }
-// out[0..5]: dynamic shared memory per CTA (with the 1 KB alignment slack), CTAs per SM, threads per CTA, and the bytes of
-// the three regions: weights + parameters, A operands + x box, tiles (T0 / T1 / conv2 staging)
-void front_tc_layout(int* out) {
-    out[0] = (int)front_tc_smem_bytes(); out[1] = 2; out[2] = FR_THREADS;
-    out[3] = (int)(FR_R1 - FR_W0 + FR_P_BYTES); out[4] = (int)(FR_R2 - FR_R1); out[5] = (int)(FR_PRM - FR_R2);
-    static_assert(FR_X + FR_X_BYTES <= FR_R2 && FR_X >= FR_R1 + FR_A0_ROWS * 128, "x box beside the stem chunk, inside the A region");
+size_t front_tc_smem_bytes(int cin) { return (size_t)fr_bar(cin) + 8 + 1024; }
+// CTAs of front_tc_kernel that fit on one SM with c_in input planes: 228 KB of shared memory per SM, 1 KB of it reserved
+// per resident CTA, and the register file (128 registers x 256 threads) caps it at two
+int front_tc_ctas_per_sm(int cin) {
+    const int c = (int)((228u * 1024u) / (front_tc_smem_bytes(cin) + 1024));
+    return c < 2 ? c : 2;
+}
+// out[0..5] for a stem of c_in planes: dynamic shared memory per CTA (with the 1 KB alignment slack), CTAs per SM, threads
+// per CTA, and the bytes of the three regions: weights + parameters, A operands + x box, tiles (T0 / T1 / conv2 staging)
+void front_tc_layout(int cin, int* out) {
+    out[0] = (int)front_tc_smem_bytes(cin); out[1] = front_tc_ctas_per_sm(cin); out[2] = FR_THREADS;
+    out[3] = (int)(FR_R1 - FR_W0 + FR_P_BYTES); out[4] = (int)(fr_r2(cin) - FR_R1); out[5] = (int)(fr_prm(cin) - fr_r2(cin));
+    static_assert(FR_X + fr_x_bytes(3) <= FR_R1 + 320 * 128 && FR_X >= FR_R1 + FR_A0_ROWS * 128,
+                  "three planes: x box beside the stem chunk, inside the A region");
+    static_assert(fr_x_over(3) == 0 && fr_x_over(4) == 2688, "c_in <= 3 keeps the layout; c_in = 4 moves the tiles up 2688 B");
 }
 
-template <typename T, bool RELU6>
+template <typename T, bool RELU6, int CIN>
 __global__ void __launch_bounds__(FR_THREADS, 2)
 front_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const FrontParams p) {
     using MF = MixFma<T>;
+    constexpr uint32_t FR_R2 = fr_r2(CIN), FR_PRM = fr_prm(CIN), FR_BAR = fr_bar(CIN), FR_X_BYTES = fr_x_bytes(CIN);
+    constexpr int KS = (9 * CIN + 15) / 16;                  // stem k16 steps
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -137,32 +155,33 @@ front_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const FrontParams p) {
         for (int ch = 0; ch < 2; ++ch) {
             if (tid < FR_A0_ROWS) {
                 const int m = ch * FR_A0_ROWS + tid;
-                uint32_t wd[16];
+                uint32_t wd[8 * KS];                       // the KS k16 steps' K positions, two per word
                 if (m < FR_T0 * FR_T0) {
                     const int ty = m / FR_T0, tx = m - ty * FR_T0;
                     // tap kx of T0 column tx is box column 2 tx + 3 + kx: the high half of word tx + 1, both halves of word tx + 2
                     const uint8_t* xs = smem + FR_X + (2 * ty * FR_XW + 2 * tx + 2) * 2;
-                    uint32_t hv[27];
+                    constexpr int NK = 9 * CIN;
+                    uint32_t hv[NK];
 #pragma unroll
-                    for (int r = 0; r < 9; ++r) {
+                    for (int r = 0; r < 3 * CIN; ++r) {
                         const int ci = r / 3, ky = r % 3;
                         const uint32_t* q = reinterpret_cast<const uint32_t*>(xs + ((ci * FR_XH + ky) * FR_XW) * 2);
                         const uint32_t v0 = q[0], v1 = q[1];
                         hv[3 * r] = v0 >> 16; hv[3 * r + 1] = v1 & 0xffffu; hv[3 * r + 2] = v1 >> 16;
                     }
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const uint32_t lo = (2 * j < 27) ? hv[(2 * j < 27) ? 2 * j : 0] : 0u;
-                        const uint32_t hi = (2 * j + 1 < 27) ? hv[(2 * j + 1 < 27) ? 2 * j + 1 : 0] : 0u;
+                    for (int j = 0; j < 8 * KS; ++j) {
+                        const uint32_t lo = (2 * j < NK) ? hv[(2 * j < NK) ? 2 * j : 0] : 0u;
+                        const uint32_t hi = (2 * j + 1 < NK) ? hv[(2 * j + 1 < NK) ? 2 * j + 1 : 0] : 0u;
                         wd[j] = lo | (hi << 16);
                     }
                 } else {
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) wd[j] = 0u;
+                    for (int j = 0; j < 8 * KS; ++j) wd[j] = 0u;
                 }
                 uint8_t* a_row = r1 + tid * 128;
 #pragma unroll
-                for (int c = 0; c < 4; ++c)
+                for (int c = 0; c < 2 * KS; ++c)
                     *reinterpret_cast<uint4*>(a_row + ((c ^ (tid & 7)) << 4)) = make_uint4(wd[4 * c], wd[4 * c + 1], wd[4 * c + 2], wd[4 * c + 3]);
             }
             fence_proxy_async();
@@ -170,8 +189,10 @@ front_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const FrontParams p) {
             for (int mb = wg; mb < 3; mb += 2) {
                 float acc[16];
                 wgmma_fence();
-                wgmma_n32<T>(acc, sw128_desc(r1_lo + (uint32_t)mb * 512u), sw128_desc(w_lo + (FR_W0 >> 4)), 0u);
-                wgmma_n32<T>(acc, sw128_desc(r1_lo + (uint32_t)mb * 512u + 2u), sw128_desc(w_lo + (FR_W0 >> 4) + 2u), 1u);
+#pragma unroll
+                for (int ks = 0; ks < KS; ++ks)
+                    wgmma_n32<T>(acc, sw128_desc(r1_lo + (uint32_t)mb * 512u + 2u * ks), sw128_desc(w_lo + (FR_W0 >> 4) + 2u * ks),
+                                 ks > 0 ? 1u : 0u);
                 wgmma_commit();
                 wgmma_wait0();
 #pragma unroll
@@ -356,19 +377,21 @@ struct FrontTcPlan {
     FrontParams p;
     dim3 grid;
     size_t smem_bytes;
-    int dtype, relu6;
+    int dtype, relu6, c_in;
     TcLaunchOpts opts;
     const void* x_bound = nullptr;
     void* blob = nullptr;
     std::string name;
 };
 
-// stages 0..2 as the kernel takes them: the stem conv_bn(3, 32, 2) with ReLU6, then two 3x3 DWPW blocks (stride 1, then 2)
-// 32 -> 64 -> 128, one act for both blocks, h and w multiples of 32 (conv2's map is whole 8x8 tiles), 16-bit.  Geometry
-// only (no driver call), so that the host-only debug export can apply the same rule.
+// stages 0..2 as the kernel takes them: the stem conv_bn(c_in, 32, 2) with ReLU6 and two CTAs per SM at that c_in (c_in
+// 1..4), then two 3x3 DWPW blocks (stride 1, then 2) 32 -> 64 -> 128, one act for both blocks, h and w multiples of 32
+// (conv2's map is whole 8x8 tiles), 16-bit.  Geometry only (no driver call), so that the host-only debug export can apply
+// the same rule.
 bool front_tc_shape_ok(int dtype, const StageGeom& g0, const StageGeom& g1, const StageGeom& g2) {
     if (dtype != FD_F16 && dtype != FD_BF16) return false;
-    if (g0.ksize != 3 || g0.stride != 2 || g0.c_in != 3 || g0.c_out != FR_C0 || g0.act != FD_ACT_RELU6 || g0.upsample) return false;
+    if (g0.ksize != 3 || g0.stride != 2 || g0.c_out != FR_C0 || g0.act != FD_ACT_RELU6 || g0.upsample) return false;
+    if (g0.c_in < 1 || g0.c_in > FR_MAX_CIN || front_tc_ctas_per_sm(g0.c_in) < 2) return false;
     if (g0.h_in % 32 || g0.w_in % 32) return false;
     if (g1.ksize != 3 || g1.stride != 1 || g1.c_in != FR_C0 || g1.c_out != FR_C1 || g1.upsample) return false;
     if (g2.ksize != 3 || g2.stride != 2 || g2.c_in != FR_C1 || g2.c_out != FR_C2 || g2.upsample) return false;
@@ -377,10 +400,10 @@ bool front_tc_shape_ok(int dtype, const StageGeom& g0, const StageGeom& g1, cons
 
 int front_tc_items(int n, int h, int w) { return n * (h / 32) * (w / 32); }
 
-// the blob: weights [224][64] 16-bit (stem [32][64] with K = (ci, ky, kx) as the stem kernel packs it, conv1 [64][64] with K
-// 32..63 zero, conv2 [128][64]), then the parameter block of the FR_P_* layout
+// the blob: weights [224][64] 16-bit (stem [32][64] with K = (ci, ky, kx) as the stem kernel packs it, zero past 9 c_in,
+// conv1 [64][64] with K 32..63 zero, conv2 [128][64]), then the parameter block of the FR_P_* layout
 template <typename T>
-__global__ void pack_front_kernel(const float* __restrict__ w27, const T* __restrict__ pw1, const T* __restrict__ pw2,
+__global__ void pack_front_kernel(int c_in, const float* __restrict__ wk, const T* __restrict__ pw1, const T* __restrict__ pw2,
                                   const float* __restrict__ sc0, const float* __restrict__ bi0,
                                   const float* __restrict__ dw1, const float* __restrict__ dsc1, const float* __restrict__ dbi1,
                                   const float* __restrict__ sc1, const float* __restrict__ bi1,
@@ -390,7 +413,7 @@ __global__ void pack_front_kernel(const float* __restrict__ w27, const T* __rest
     T* wt = reinterpret_cast<T*>(blob);
     if (i < (FR_C0 + FR_C1 + FR_C2) * 64) {
         const int r = i / 64, k = i % 64;
-        if (r < FR_C0) wt[i] = Traits<T>::from_f(k < 27 ? w27[k * FR_C0 + r] : 0.f);
+        if (r < FR_C0) wt[i] = Traits<T>::from_f(k < 9 * c_in ? wk[k * FR_C0 + r] : 0.f);
         else if (r < FR_C0 + FR_C1) wt[i] = k < FR_C0 ? pw1[(r - FR_C0) * FR_C0 + k] : Traits<T>::from_f(0.f);
         else wt[i] = pw2[(r - FR_C0 - FR_C1) * FR_C1 + k];
     }
@@ -419,9 +442,10 @@ static int encode_front_x(FrontTcPlan* fp, const void* x) {
     PFN_encodeTiled encode = get_tensor_map_encoder();
     const CUtensorMapDataType dt = fp->dtype == FD_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     const FrontParams& p = fp->p;
-    cuuint64_t dims[4] = {(cuuint64_t)p.w, (cuuint64_t)p.h, 3, (cuuint64_t)p.n};
-    cuuint64_t strides[3] = {(cuuint64_t)p.w * 2, (cuuint64_t)p.w * p.h * 2, (cuuint64_t)p.w * p.h * 6};
-    cuuint32_t box[4] = {FR_XW, FR_XH, 3, 1};
+    const cuuint64_t plane = (cuuint64_t)p.w * p.h * 2;
+    cuuint64_t dims[4] = {(cuuint64_t)p.w, (cuuint64_t)p.h, (cuuint64_t)fp->c_in, (cuuint64_t)p.n};
+    cuuint64_t strides[3] = {(cuuint64_t)p.w * 2, plane, plane * (cuuint64_t)fp->c_in};
+    cuuint32_t box[4] = {FR_XW, FR_XH, (cuuint32_t)fp->c_in, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = encode(&fp->tm_x, dt, 4, const_cast<void*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -430,12 +454,12 @@ static int encode_front_x(FrontTcPlan* fp, const void* x) {
     return FD_OK;
 }
 
-int front_tc_prepare(int dtype, const StageGeom& g0, const StageGeom& g1, const StageGeom& g2, const float* w27,
+int front_tc_prepare(int dtype, const StageGeom& g0, const StageGeom& g1, const StageGeom& g2, const float* wk,
                      const float* sc0, const float* bi0, const BlockArgs& a1, const BlockArgs& a2, void* out0,
                      const TcLaunchOpts& opts, FrontTcPlan** res) {
     FrontTcPlan* fp = new (std::nothrow) FrontTcPlan();
     if (!fp) return fail(FD_ERR_CUDA, "out of host memory");
-    fp->dtype = dtype; fp->relu6 = g1.act == FD_ACT_RELU6; fp->opts = opts;
+    fp->dtype = dtype; fp->relu6 = g1.act == FD_ACT_RELU6; fp->c_in = g0.c_in; fp->opts = opts;
     FrontParams& p = fp->p;
     memset(&p, 0, sizeof(p));
     p.n = g0.n; p.h = g0.h_in; p.w = g0.w_in;
@@ -446,11 +470,11 @@ int front_tc_prepare(int dtype, const StageGeom& g0, const StageGeom& g1, const 
     if (cudaMalloc(&fp->blob, blob_bytes) != cudaSuccess) { front_tc_destroy(fp); return fail(FD_ERR_CUDA, "cudaMalloc failed"); }
     const int tot = (FR_C0 + FR_C1 + FR_C2) * 64;
     if (dtype == FD_F16)
-        pack_front_kernel<__half><<<(tot + 127) / 128, 128>>>(w27, (const __half*)a1.pw_w, (const __half*)a2.pw_w, sc0, bi0, a1.dw_w, a1.dw_scale,
+        pack_front_kernel<__half><<<(tot + 127) / 128, 128>>>(g0.c_in, wk, (const __half*)a1.pw_w, (const __half*)a2.pw_w, sc0, bi0, a1.dw_w, a1.dw_scale,
                                                               a1.dw_bias, a1.pw_scale, a1.pw_bias, a2.dw_w, a2.dw_scale, a2.dw_bias,
                                                               a2.pw_scale, a2.pw_bias, (uint8_t*)fp->blob);
     else
-        pack_front_kernel<__nv_bfloat16><<<(tot + 127) / 128, 128>>>(w27, (const __nv_bfloat16*)a1.pw_w, (const __nv_bfloat16*)a2.pw_w, sc0, bi0,
+        pack_front_kernel<__nv_bfloat16><<<(tot + 127) / 128, 128>>>(g0.c_in, wk, (const __nv_bfloat16*)a1.pw_w, (const __nv_bfloat16*)a2.pw_w, sc0, bi0,
                                                                      a1.dw_w, a1.dw_scale, a1.dw_bias, a1.pw_scale, a1.pw_bias, a2.dw_w,
                                                                      a2.dw_scale, a2.dw_bias, a2.pw_scale, a2.pw_bias, (uint8_t*)fp->blob);
     if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) {
@@ -458,10 +482,11 @@ int front_tc_prepare(int dtype, const StageGeom& g0, const StageGeom& g1, const 
         return fail(FD_ERR_CUDA, "front parameter packing failed");
     }
     p.blob = reinterpret_cast<const uint4*>(fp->blob);
-    fp->smem_bytes = front_tc_smem_bytes();
+    fp->smem_bytes = front_tc_smem_bytes(g0.c_in);
     const int ctas = 2 * opts.n_sms;
     fp->grid = dim3((unsigned)(p.items < ctas ? p.items : ctas), 1, 1);
-    fp->name = std::string("stem_tc+front<k3s1,k3s2,8x8>[n32,n64,n128,") + (fp->relu6 ? "relu6]" : "relu]");
+    fp->name = std::string("stem_tc+front<k3s1,k3s2,8x8>[n32,n64,n128,") + (fp->relu6 ? "relu6" : "relu") +
+               (g0.c_in == 3 ? "]" : ",cin" + std::to_string(g0.c_in) + "]");
     *res = fp;
     return FD_OK;
 }
@@ -469,17 +494,28 @@ int front_tc_prepare(int dtype, const StageGeom& g0, const StageGeom& g1, const 
 size_t front_tc_param_bytes(FrontTcPlan*) { return FR_W_BYTES + FR_P_BYTES; }
 const char* front_tc_name(FrontTcPlan* fp) { return fp->name.c_str(); }
 
-template <typename T, bool R6>
+template <typename T, bool R6, int CIN>
 static int launch_front(FrontTcPlan* fp, cudaLaunchConfig_t& cfg) {
     static PerDeviceOnce attr_done;
     int dev = -1;
     FD_CUDA_OK(cudaGetDevice(&dev));
     if (attr_done.need(dev)) {
-        FD_CUDA_OK(cudaFuncSetAttribute(front_tc_kernel<T, R6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fp->smem_bytes));
+        FD_CUDA_OK(cudaFuncSetAttribute(front_tc_kernel<T, R6, CIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fp->smem_bytes));
         attr_done.done(dev);
     }
-    FD_CUDA_OK(cudaLaunchKernelEx(&cfg, front_tc_kernel<T, R6>, fp->tm_x, fp->p));
+    FD_CUDA_OK(cudaLaunchKernelEx(&cfg, front_tc_kernel<T, R6, CIN>, fp->tm_x, fp->p));
     return FD_OK;
+}
+
+template <typename T, bool R6>
+static int launch_front_cin(FrontTcPlan* fp, cudaLaunchConfig_t& cfg) {
+    switch (fp->c_in) {
+        case 1: return launch_front<T, R6, 1>(fp, cfg);
+        case 2: return launch_front<T, R6, 2>(fp, cfg);
+        case 3: return launch_front<T, R6, 3>(fp, cfg);
+        case 4: return launch_front<T, R6, 4>(fp, cfg);
+        default: return fail(FD_ERR_UNSUPPORTED, "front_tc_kernel: c_in must be 1..4");
+    }
 }
 
 // x may change from call to call: the input tensor map is re-encoded when it does (as stem_tc_launch)
@@ -496,8 +532,8 @@ int front_tc_launch(FrontTcPlan* fp, const void* x, cudaStream_t st) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = fp->opts.pdl ? 1 : 0;
     int rc;
-    if (fp->dtype == FD_F16) rc = fp->relu6 ? launch_front<__half, true>(fp, cfg) : launch_front<__half, false>(fp, cfg);
-    else rc = fp->relu6 ? launch_front<__nv_bfloat16, true>(fp, cfg) : launch_front<__nv_bfloat16, false>(fp, cfg);
+    if (fp->dtype == FD_F16) rc = fp->relu6 ? launch_front_cin<__half, true>(fp, cfg) : launch_front_cin<__half, false>(fp, cfg);
+    else rc = fp->relu6 ? launch_front_cin<__nv_bfloat16, true>(fp, cfg) : launch_front_cin<__nv_bfloat16, false>(fp, cfg);
     if (rc) return rc;
     FD_CUDA_OK(cudaGetLastError());
     return FD_OK;

@@ -1,6 +1,7 @@
 // SIMT kernels of the FastDepth forward path (all dtypes).
 //
-//  * stem_kernel  : conv_bn(3,C0,s2)+BN+ReLU6, NCHW in -> NHWC out   (reference imagenet/mobilenet.py:22-27,41)
+//  * stem_kernel  : conv_bn(c_in,C0,s2)+BN+ReLU6, NCHW in -> NHWC out, c_in 1..7
+//                                                                      (reference imagenet/mobilenet.py:22-27,41; models.py:443-453)
 //  * dw_kernel    : depthwise kxk(stride)+BN+act, NHWC                (reference imagenet/mobilenet.py:31-33; models.py:61-68)
 //  * pw_kernel    : pointwise 1x1+BN+act as a tiled SIMT GEMM, with the decoder's nearest-x2
 //                   upsample + skip add in the epilogue               (reference imagenet/mobilenet.py:35-37; models.py:70-75,723-729)
@@ -23,13 +24,13 @@ namespace fd {
 // ----------------------------------------------------------------------------------------
 // stem
 // ----------------------------------------------------------------------------------------
-template <typename T>
+template <typename T, int CIN>
 __global__ void __launch_bounds__(256)
 stem_kernel(const T* __restrict__ x, T* __restrict__ out, const float* __restrict__ w,
             const float* __restrict__ scale, const float* __restrict__ bias,
             int n, int h_in, int w_in, int h_out, int w_out, int c_out, int out_pitch, int stride, int act) {
-    extern __shared__ float s_w[];                 // [27][c_out] tap-major, then scale, bias
-    const int nw = 27 * c_out;
+    extern __shared__ float s_w[];                 // [9 c_in][c_out] tap-major, then scale, bias
+    const int nw = 9 * CIN * c_out;
     for (int i = threadIdx.x; i < nw; i += blockDim.x) s_w[i] = w[i];
     float* s_scale = s_w + nw;
     float* s_bias = s_scale + c_out;
@@ -50,9 +51,9 @@ stem_kernel(const T* __restrict__ x, T* __restrict__ out, const float* __restric
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] = 0.f;
     const size_t plane = (size_t)h_in * w_in;
-    const T* xi = x + (size_t)img * 3 * plane;
+    const T* xi = x + (size_t)img * CIN * plane;
 #pragma unroll
-    for (int ci = 0; ci < 3; ++ci) {
+    for (int ci = 0; ci < CIN; ++ci) {
 #pragma unroll
         for (int ky = 0; ky < 3; ++ky) {
             const int iy = oy * stride - 1 + ky;
@@ -449,9 +450,21 @@ static int launch_stem_t(const void* x, void* out, const float* w, const float* 
     const long long total = (long long)g.n * g.h_out * g.w_out * (g.c_out / 8);
     const int threads = 256;
     const long long blocks = (total + threads - 1) / threads;
-    const size_t smem = (size_t)(27 + 2) * g.c_out * sizeof(float);
-    stem_kernel<T><<<(unsigned)blocks, threads, smem, st>>>((const T*)x, (T*)out, w, scale, bias, g.n, g.h_in, g.w_in,
-                                                           g.h_out, g.w_out, g.c_out, g.out_pitch, g.stride, g.act);
+    const size_t smem = (size_t)(9 * g.c_in + 2) * g.c_out * sizeof(float);
+    decltype(&stem_kernel<T, 3>) k;
+    switch (g.c_in) {
+        case 1: k = stem_kernel<T, 1>; break;
+        case 2: k = stem_kernel<T, 2>; break;
+        case 3: k = stem_kernel<T, 3>; break;
+        case 4: k = stem_kernel<T, 4>; break;
+        case 5: k = stem_kernel<T, 5>; break;
+        case 6: k = stem_kernel<T, 6>; break;
+        case 7: k = stem_kernel<T, 7>; break;
+        default: return fail(FD_ERR_UNSUPPORTED, "stem_kernel: c_in must be 1..7");
+    }
+    if (smem > 48 * 1024) FD_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k<<<(unsigned)blocks, threads, smem, st>>>((const T*)x, (T*)out, w, scale, bias, g.n, g.h_in, g.w_in, g.h_out, g.w_out,
+                                               g.c_out, g.out_pitch, g.stride, g.act);
     FD_CUDA_OK(cudaGetLastError());
     return FD_OK;
 }

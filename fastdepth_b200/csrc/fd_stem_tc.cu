@@ -1,14 +1,16 @@
-// Stem (conv_bn(3, C0, stride 2) + BN + ReLU6, reference imagenet/mobilenet.py:22-27, 41) on wgmma.
+// Stem (conv_bn(c_in, C0, stride 2) + BN + ReLU6, reference imagenet/mobilenet.py:22-27, 41 and models.py:443-453) on
+// wgmma, for 1 <= c_in <= 7 input channels (RGB: 3, depth only: 1, RGB-D: 4).
 //
-// A dense 3x3x3 convolution is a K = 27 contraction per output pixel: on SIMT that is 27*C0 FMAs per pixel
-// (694 MMAC per batch of 64, more than twice the HBM time of the stage), on the tensor core it is a
-// M=128 x N=C0 x K=32 product per 128-pixel tile once the im2col rows sit in shared memory.  So:
-//   warp 8     TMA producer : 4-D box [1 img][3 planes][17 rows][40 cols] of the NCHW input per 8x16 output tile
+// A dense 3x3 convolution over c_in planes is a K = 9*c_in contraction per output pixel: on SIMT that is 27*C0 FMAs per
+// pixel at c_in = 3 (694 MMAC per batch of 64, more than twice the HBM time of the stage), on the tensor core it is a
+// M=128 x N=C0 x K=16*ceil(9*c_in/16) product per 128-pixel tile once the im2col rows sit in shared memory.  9*c_in <= 63,
+// so one pixel's im2col row is one 128-byte SW128 K-major row for every c_in.  So:
+//   warp 8     TMA producer : 4-D box [1 img][c_in planes][17 rows][40 cols] of the NCHW input per 8x16 output tile
 //                             (OOB zero fill == the conv's zero padding); stem weights [C0pad x 64] loaded once
-//   warps 0-3  im2col       : thread = output pixel; gathers its 27 taps from the staged planes and writes the
-//                             128B-swizzled K-major A row (K padded to 32 with zeros)
-//   warps 4-7  consumer     : one warpgroup: wgmma m64n32k16 (two row halves x C0 / 32 column blocks x two K steps) into
-//                             register accumulators -> BN affine + ReLU6 -> 16-bit NHWC store
+//   warps 0-3  im2col       : thread = output pixel; gathers its 9*c_in taps from the staged planes and writes the
+//                             128B-swizzled K-major A row, K = ci*9 + ky*3 + kx, zero past 9*c_in
+//   warps 4-7  consumer     : one warpgroup: wgmma m64n32k16 (two row halves x C0 / 32 column blocks x ceil(9*c_in/16)
+//                             K steps: 2 at c_in = 3) into register accumulators -> BN affine + ReLU6 -> 16-bit NHWC store
 // Persistent: one CTA per SM walks tiles blockIdx.x, +gridDim.x, ...
 #include <cstdio>
 #include <cstring>
@@ -25,8 +27,10 @@ constexpr int ST_TH = 8, ST_TW = 16;
 constexpr int ST_IH = 17, ST_IW = 40;                 // rows 2*7+3 = 17; cols: the 33 needed ones sit at box columns 7..39 because
                                                       // the box starts 8 elements (16 bytes) left of column 2*ox0 (aligned start)
 constexpr int ST_XSHIFT = 8;
-constexpr int ST_IN_BYTES = 3 * ST_IH * ST_IW * 2;    // 4080
-constexpr int ST_IN_STRIDE = 4096;
+constexpr int ST_MAX_CIN = 7;                        // K = 9*c_in fits one 64-element K-major row
+__host__ __device__ constexpr int st_in_bytes(int cin) { return cin * ST_IH * ST_IW * 2; }                  // 4080 at c_in = 3
+__host__ __device__ constexpr int st_in_stride(int cin) { return (st_in_bytes(cin) + 1023) / 1024 * 1024; } // 4096 at c_in = 3
+__host__ __device__ constexpr int st_ksteps(int cin) { return (9 * cin + 15) / 16; }                        // k16 steps: 2 at c_in = 3
 constexpr int ST_A_BYTES = 128 * 128;
 constexpr int ST_S_IN = 8, ST_S_A = 3;
 
@@ -45,10 +49,11 @@ struct StemBarriers {
     uint64_t b_full;
 };
 
-template <typename T>
+template <typename T, int CIN>
 __global__ void __launch_bounds__(ST_THREADS, 1)
 stem_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w, const StemParams p) {
     using MF = MixFma<T>;
+    constexpr int ST_IN_BYTES = st_in_bytes(CIN), ST_IN_STRIDE = st_in_stride(CIN), KS = st_ksteps(CIN);
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -69,7 +74,7 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
     }
     if (warp == ST_WARP_TMA && lane == 0) { tma_prefetch_desc(&tm_in); tma_prefetch_desc(&tm_w); }
     for (int i = threadIdx.x; i < p.n_pad; i += ST_THREADS) s_affine[i] = p.affine[i];
-    // the K = 32..63 half of every A row is never read (only two K=16 steps are issued), no need to clear it
+    // an A row gets the K positions its KS k16 steps read (zeros past 9*c_in); the rest of the 128-byte row is never read
     pdl_launch_dependents();                       // the next kernel may begin its own prologue
     pdl_wait_prior_grid();                         // everything below reads what the previous kernel wrote
     __syncthreads();
@@ -104,10 +109,11 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
             mbar_wait(smem_u32(&bars->in_full[rin.s]), rin.ph);
             // tap kx of pixel tx is box column 2*tx + kx + 7: words (tx+3) [high half] and (tx+4) [both halves]
             const uint8_t* in_s = smem + in_off + rin.s * ST_IN_STRIDE + (2 * ty * ST_IW + 2 * tx + ST_XSHIFT - 2) * 2;
-            // 9 (plane, ky) rows of 3 taps from two aligned 32-bit words
-            uint32_t h[27];
+            // 3*c_in (plane, ky) rows of 3 taps from two aligned 32-bit words
+            constexpr int NK = 9 * CIN;
+            uint32_t h[NK];
 #pragma unroll
-            for (int r = 0; r < 9; ++r) {
+            for (int r = 0; r < 3 * CIN; ++r) {
                 const int ci = r / 3, ky = r % 3;
                 const uint32_t* q = reinterpret_cast<const uint32_t*>(in_s + ((ci * ST_IH + ky) * ST_IW) * 2);
                 const uint32_t w0 = q[0], w1 = q[1];
@@ -115,17 +121,17 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(smem_u32(&bars->in_empty[rin.s]));
-            uint32_t wd[16];
+            uint32_t wd[8 * KS];                       // the KS k16 steps' K positions, two per word
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const uint32_t lo = (2 * j < 27) ? h[(2 * j < 27) ? 2 * j : 0] : 0u;
-                const uint32_t hi = (2 * j + 1 < 27) ? h[(2 * j + 1 < 27) ? 2 * j + 1 : 0] : 0u;
+            for (int j = 0; j < 8 * KS; ++j) {
+                const uint32_t lo = (2 * j < NK) ? h[(2 * j < NK) ? 2 * j : 0] : 0u;
+                const uint32_t hi = (2 * j + 1 < NK) ? h[(2 * j + 1 < NK) ? 2 * j + 1 : 0] : 0u;
                 wd[j] = lo | (hi << 16);
             }
             mbar_wait(smem_u32(&bars->a_empty[ra.s]), ra.ph ^ 1u);
             uint8_t* a_row = smem + a_off + ra.s * ST_A_BYTES + m * 128;
 #pragma unroll
-            for (int c = 0; c < 4; ++c)
+            for (int c = 0; c < 2 * KS; ++c)
                 *reinterpret_cast<uint4*>(a_row + ((c ^ (m & 7)) << 4)) = make_uint4(wd[4 * c], wd[4 * c + 1], wd[4 * c + 2], wd[4 * c + 3]);
             fence_proxy_async();
             __syncwarp();
@@ -150,9 +156,11 @@ stem_tc_kernel(const __grid_constant__ CUtensorMap tm_in, const __grid_constant_
             for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
                 for (int j = 0; j < ST_MAX_N / 32; ++j) {
-                    if (j < nch) {                        // K = 32: two steps of 16 (+32 B each); B rows of block j at +j * 4 KB
-                        wgmma_n32<T>(acc[mh][j], sw128_desc(a_lo + (uint32_t)mh * 512u), sw128_desc(b_lo + (uint32_t)j * 256u), 0u);
-                        wgmma_n32<T>(acc[mh][j], sw128_desc(a_lo + (uint32_t)mh * 512u + 2u), sw128_desc(b_lo + (uint32_t)j * 256u + 2u), 1u);
+                    if (j < nch) {                        // KS steps of 16 (+32 B each) from a zero accumulator; B rows of block j at +j * 4 KB
+#pragma unroll
+                        for (int ks = 0; ks < KS; ++ks)
+                            wgmma_n32<T>(acc[mh][j], sw128_desc(a_lo + (uint32_t)mh * 512u + 2u * ks),
+                                         sw128_desc(b_lo + (uint32_t)j * 256u + 2u * ks), ks > 0 ? 1u : 0u);
                     }
                 }
             wgmma_commit();
@@ -190,7 +198,7 @@ struct StemTcPlan {
     StemParams p;
     dim3 grid;
     size_t smem_bytes;
-    int dtype;
+    int dtype, c_in;
     TcLaunchOpts opts;
     const void* x_bound = nullptr;       // input pointer the tensor map was encoded for
     void* w16 = nullptr;                 // [n_pad][64] 16-bit, K = (ci, ky, kx) padded
@@ -200,11 +208,11 @@ struct StemTcPlan {
 };
 
 template <typename T>
-__global__ void pack_stem_w_kernel(const float* __restrict__ w27, T* __restrict__ dst, int c_out, int n_pad) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;           // dst[co][k], src tap-major [k][c_out]
+__global__ void pack_stem_w_kernel(const float* __restrict__ wk, T* __restrict__ dst, int c_in, int c_out, int n_pad) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;           // dst[co][k], src tap-major [9 c_in][c_out]
     if (i >= n_pad * 64) return;
     const int co = i / 64, k = i % 64;
-    dst[i] = Traits<T>::from_f((co < c_out && k < 27) ? w27[k * c_out + co] : 0.f);
+    dst[i] = Traits<T>::from_f((co < c_out && k < 9 * c_in) ? wk[k * c_out + co] : 0.f);
 }
 __global__ void pack_stem_affine_kernel(const float* __restrict__ scale, const float* __restrict__ bias, float2* __restrict__ dst,
                                         int c_out, int n_pad) {
@@ -219,7 +227,7 @@ __global__ void pack_stem_affine_kernel(const float* __restrict__ scale, const f
 
 bool stem_tc_supported(int dtype, const StageGeom& g) {
     if (dtype != FD_F16 && dtype != FD_BF16) return false;
-    if (g.ksize != 3 || g.stride != 2 || g.c_in != 3 || g.act != FD_ACT_RELU6) return false;
+    if (g.ksize != 3 || g.stride != 2 || g.c_in < 1 || g.c_in > ST_MAX_CIN || g.act != FD_ACT_RELU6) return false;
     if (g.c_out % 8 || g.c_out > ST_MAX_N || (g.w_in % 8)) return false;       // W*2 bytes must be a 16-byte multiple for TMA
     return get_tensor_map_encoder() != nullptr;
 }
@@ -233,9 +241,10 @@ void stem_tc_destroy(StemTcPlan* sp) {
 static int encode_input_map(StemTcPlan* sp, const void* x) {
     PFN_encodeTiled encode = get_tensor_map_encoder();
     const CUtensorMapDataType dt = sp->dtype == FD_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-    cuuint64_t dims[4] = {(cuuint64_t)sp->w_in, (cuuint64_t)sp->h_in, 3, (cuuint64_t)sp->n};
-    cuuint64_t strides[3] = {(cuuint64_t)sp->w_in * 2, (cuuint64_t)sp->w_in * sp->h_in * 2, (cuuint64_t)sp->w_in * sp->h_in * 6};
-    cuuint32_t box[4] = {ST_IW, ST_IH, 3, 1};
+    const cuuint64_t plane = (cuuint64_t)sp->w_in * sp->h_in * 2;
+    cuuint64_t dims[4] = {(cuuint64_t)sp->w_in, (cuuint64_t)sp->h_in, (cuuint64_t)sp->c_in, (cuuint64_t)sp->n};
+    cuuint64_t strides[3] = {(cuuint64_t)sp->w_in * 2, plane, plane * (cuuint64_t)sp->c_in};
+    cuuint32_t box[4] = {ST_IW, ST_IH, (cuuint32_t)sp->c_in, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = encode(&sp->tm_in, dt, 4, const_cast<void*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -244,13 +253,13 @@ static int encode_input_map(StemTcPlan* sp, const void* x) {
     return FD_OK;
 }
 
-int stem_tc_prepare(int dtype, const StageGeom& g, const float* w27_dev, const float* scale_dev, const float* bias_dev, void* out,
+int stem_tc_prepare(int dtype, const StageGeom& g, const float* wk_dev, const float* scale_dev, const float* bias_dev, void* out,
                     const TcLaunchOpts& opts, StemTcPlan** res) {
     PFN_encodeTiled encode = get_tensor_map_encoder();
     if (!encode) return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     StemTcPlan* sp = new (std::nothrow) StemTcPlan();
     if (!sp) return fail(FD_ERR_CUDA, "out of host memory");
-    sp->dtype = dtype; sp->n = g.n; sp->h_in = g.h_in; sp->w_in = g.w_in;
+    sp->dtype = dtype; sp->c_in = g.c_in; sp->n = g.n; sp->h_in = g.h_in; sp->w_in = g.w_in;
     StemParams& p = sp->p;
     memset(&p, 0, sizeof(p));
     p.n = g.n; p.h_in = g.h_in; p.w_in = g.w_in; p.h_out = g.h_out; p.w_out = g.w_out; p.c_out = g.c_out;
@@ -266,8 +275,8 @@ int stem_tc_prepare(int dtype, const StageGeom& g, const float* w27_dev, const f
         rc = fail(FD_ERR_CUDA, "cudaMalloc failed");
     if (rc == FD_OK) {
         const int tot = p.n_pad * 64;
-        if (dtype == FD_F16) pack_stem_w_kernel<__half><<<(tot + 127) / 128, 128>>>(w27_dev, (__half*)sp->w16, g.c_out, p.n_pad);
-        else pack_stem_w_kernel<__nv_bfloat16><<<(tot + 127) / 128, 128>>>(w27_dev, (__nv_bfloat16*)sp->w16, g.c_out, p.n_pad);
+        if (dtype == FD_F16) pack_stem_w_kernel<__half><<<(tot + 127) / 128, 128>>>(wk_dev, (__half*)sp->w16, g.c_in, g.c_out, p.n_pad);
+        else pack_stem_w_kernel<__nv_bfloat16><<<(tot + 127) / 128, 128>>>(wk_dev, (__nv_bfloat16*)sp->w16, g.c_in, g.c_out, p.n_pad);
         pack_stem_affine_kernel<<<(p.n_pad + 127) / 128, 128>>>(scale_dev, bias_dev, sp->affine, g.c_out, p.n_pad);
         if (cudaGetLastError() != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) rc = fail(FD_ERR_CUDA, "stem parameter packing failed");
     }
@@ -283,13 +292,14 @@ int stem_tc_prepare(int dtype, const StageGeom& g, const float* w27_dev, const f
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { stem_tc_destroy(sp); return fail(FD_ERR_CUDA, "cuTensorMapEncodeTiled(stem weights) failed"); }
     }
-    sp->smem_bytes = (size_t)ST_S_A * ST_A_BYTES + (size_t)p.n_pad * 128 + (size_t)ST_S_IN * ST_IN_STRIDE + (size_t)p.n_pad * 8 +
+    sp->smem_bytes = (size_t)ST_S_A * ST_A_BYTES + (size_t)p.n_pad * 128 + (size_t)ST_S_IN * st_in_stride(g.c_in) + (size_t)p.n_pad * 8 +
                      sizeof(StemBarriers) + 1024;
     const int sms = opts.n_sms;
     sp->opts = opts;
     sp->grid = dim3((unsigned)(p.items < sms ? p.items : sms), 1, 1);
     char buf[96];
-    snprintf(buf, sizeof(buf), "stem_tc<k3,s2,1x8x16>[n%d]", p.n_pad);
+    if (g.c_in == 3) snprintf(buf, sizeof(buf), "stem_tc<k3,s2,1x8x16>[n%d]", p.n_pad);
+    else snprintf(buf, sizeof(buf), "stem_tc<k3,s2,1x8x16,cin%d>[n%d]", g.c_in, p.n_pad);
     sp->name = buf;
     *res = sp;
     return FD_OK;
@@ -297,6 +307,33 @@ int stem_tc_prepare(int dtype, const StageGeom& g, const float* w27_dev, const f
 
 size_t stem_tc_param_bytes(StemTcPlan* sp) { return (size_t)sp->p.n_pad * (64 * 2 + sizeof(float2)); }
 const char* stem_tc_name(StemTcPlan* sp) { return sp->name.c_str(); }
+
+template <typename T, int CIN>
+static int launch_stem_tc(StemTcPlan* sp, cudaLaunchConfig_t& cfg) {
+    static PerDeviceOnce attr_done;            // the dynamic shared-memory opt-in is per device and per kernel instance
+    int dev = -1;
+    FD_CUDA_OK(cudaGetDevice(&dev));
+    if (attr_done.need(dev)) {
+        FD_CUDA_OK(cudaFuncSetAttribute(stem_tc_kernel<T, CIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        attr_done.done(dev);
+    }
+    FD_CUDA_OK(cudaLaunchKernelEx(&cfg, stem_tc_kernel<T, CIN>, sp->tm_in, sp->tm_w, sp->p));
+    return FD_OK;
+}
+
+template <typename T>
+static int launch_stem_cin(StemTcPlan* sp, cudaLaunchConfig_t& cfg) {
+    switch (sp->c_in) {
+        case 1: return launch_stem_tc<T, 1>(sp, cfg);
+        case 2: return launch_stem_tc<T, 2>(sp, cfg);
+        case 3: return launch_stem_tc<T, 3>(sp, cfg);
+        case 4: return launch_stem_tc<T, 4>(sp, cfg);
+        case 5: return launch_stem_tc<T, 5>(sp, cfg);
+        case 6: return launch_stem_tc<T, 6>(sp, cfg);
+        case 7: return launch_stem_tc<T, 7>(sp, cfg);
+        default: return fail(FD_ERR_UNSUPPORTED, "stem_tc_kernel: c_in must be 1..7");
+    }
+}
 
 // x may change from call to call (the caller's tensor): re-encode the input tensor map when it does.  Under CUDA-graph
 // capture the map is baked into the captured launch, which is keyed on (x, y) by the caller.
@@ -312,16 +349,10 @@ int stem_tc_launch(StemTcPlan* sp, const void* x, cudaStream_t st) {
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = sp->opts.pdl ? 1 : 0;
-    static PerDeviceOnce attr_done[2];         // the dynamic shared-memory opt-in is per device and per kernel instance
-    int dev = -1;
-    FD_CUDA_OK(cudaGetDevice(&dev));
-    if (sp->dtype == FD_F16) {
-        if (attr_done[0].need(dev)) { FD_CUDA_OK(cudaFuncSetAttribute(stem_tc_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); attr_done[0].done(dev); }
-        FD_CUDA_OK(cudaLaunchKernelEx(&cfg, stem_tc_kernel<__half>, sp->tm_in, sp->tm_w, sp->p));
-    } else {
-        if (attr_done[1].need(dev)) { FD_CUDA_OK(cudaFuncSetAttribute(stem_tc_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); attr_done[1].done(dev); }
-        FD_CUDA_OK(cudaLaunchKernelEx(&cfg, stem_tc_kernel<__nv_bfloat16>, sp->tm_in, sp->tm_w, sp->p));
-    }
+    int rc;
+    if (sp->dtype == FD_F16) rc = launch_stem_cin<__half>(sp, cfg);
+    else rc = launch_stem_cin<__nv_bfloat16>(sp, cfg);
+    if (rc) return rc;
     FD_CUDA_OK(cudaGetLastError());
     return FD_OK;
 }

@@ -11,7 +11,7 @@ under the default ``'highest'`` they stay on the fp32 SIMT kernels.  An explicit
 precision setting.  ``models.MobileNet`` hands an fp32 input with a dense decoder to the engine only under ``'high'`` or
 ``'medium'``: split TF32 stays within the fp32 bound of 1e-3 where cuDNN's plain TF32 convs do not.
 
-One plan per (device, dtype) is live at a time.  A request [n,3,h,w] whose pixels n*h*w fit the plan's capacity (the
+One plan per (device, dtype) is live at a time.  A request [n,c_in,h,w] (c_in the stem's input channels, 1..7) whose pixels n*h*w fit the plan's capacity (the
 n*h*w it was built for) runs on it, whatever its batch size and resolution (the C-ABI builds the steps for that shape once,
 over the plan's buffers and weights; ``fd_forward_shape``).  A larger request replaces it with a plan built for the
 request's own shape, whose capacity covers everything the old one served.  So an evaluation with a short last batch, or a
@@ -79,9 +79,13 @@ class SkipAddEngine:
         if not x.is_cuda:
             raise RuntimeError("fastdepth_b200: the accelerated forward needs a CUDA tensor; "
                                "there is no CPU fallback (use models.MobileNet for CPU plumbing)")
-        if x.dim() != 4 or x.shape[1] != 3:
-            raise RuntimeError("expected input [N,3,H,W], got %s" % (tuple(x.shape),))
-        wdtype = _plan._blocks_of(m)[0][0][0].weight.dtype
+        stem_w = _plan._blocks_of(m)[0][0][0].weight
+        if x.dim() != 4:
+            raise RuntimeError("expected input [N,%d,H,W], got %s" % (stem_w.shape[1], tuple(x.shape)))
+        if x.shape[1] != stem_w.shape[1]:
+            raise RuntimeError("Given groups=1, weight of size %s, expected input%s to have %d channels, but got %d channels "
+                               "instead" % (list(stem_w.shape), list(x.shape), stem_w.shape[1], x.shape[1]))
+        wdtype = stem_w.dtype
         if x.dtype != wdtype:
             raise RuntimeError("Input type (%s) and weight type (%s) should be the same" % (x.dtype, wdtype))
         if x.dtype not in _SUPPORTED:

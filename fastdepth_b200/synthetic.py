@@ -42,7 +42,14 @@ BETA = (0.6, 0.25)
 HOT = (0.02, 2.5, 3.5)      # fraction of encoder channels with a large gamma (drives the ReLU6 clamp)
 
 
-def synthetic_state_dict(widths=STOCK_WIDTHS, seed=1, calib_hw=(96, 128), skip='add', recipe='hot'):
+def _probe(seed, calib_hw, in_channels):
+    """The seeded calibration batch: 2 images of ``in_channels`` channels (3: the fixtures' original draw, unchanged)."""
+    if in_channels == 3:
+        return torch.from_numpy(np.random.Generator(np.random.PCG64(seed + 7919)).random((2, 3) + tuple(calib_hw)))
+    return synthetic_input(2, calib_hw[0], calib_hw[1], seed=seed + 7919, channels=in_channels).double()
+
+
+def synthetic_state_dict(widths=STOCK_WIDTHS, seed=1, calib_hw=(96, 128), skip='add', recipe='hot', in_channels=3):
     """state_dict (torch fp32 CPU tensors) with the MobileNetSkipAdd key schema
     (SURVEY.md section 8a-a2).
 
@@ -56,11 +63,15 @@ def synthetic_state_dict(widths=STOCK_WIDTHS, seed=1, calib_hw=(96, 128), skip='
 
     ``recipe='calm'`` is the same recipe WITHOUT the hot channels: no single element's storage noise is amplified
     ~4x, so every intermediate stage can be held to the end-to-end tolerance (1e-2 in fp16) and a stage bug of a few
-    percent cannot hide behind the loose stage bound the hot recipe needs (tests/test_gpu_parity.py)."""
+    percent cannot hide behind the loose stage bound the hot recipe needs (tests/test_gpu_parity.py).
+
+    ``in_channels`` (reference ``MobileNet(..., in_channels)``, models.py:443-453) sets the stem's input channels: its
+    weights are drawn as [enc[0], in_channels, 3, 3] and the probe batch is ``synthetic_input(..., channels=in_channels)``.
+    With the default 3 every draw is the one above, so the existing fixtures stay bit-identical."""
     if recipe not in ('hot', 'calm'):
         raise ValueError('recipe must be "hot" or "calm"')
     hot_cfg = HOT if recipe == 'hot' else (0.0, HOT[1], HOT[2])
-    key = (tuple(widths[0]), tuple(widths[1]), int(seed), tuple(calib_hw), GAMMA_RANGE, BETA, hot_cfg, skip)
+    key = (tuple(widths[0]), tuple(widths[1]), int(seed), tuple(calib_hw), GAMMA_RANGE, BETA, hot_cfg, skip, int(in_channels))
     if key in _CACHE:
         return {k: v.clone() for k, v in _CACHE[key].items()}
     import torch.nn.functional as F
@@ -101,8 +112,9 @@ def synthetic_state_dict(widths=STOCK_WIDTHS, seed=1, calib_hw=(96, 128), skip='
         return sd[name].to(f64)
 
     strides = (2, 1, 2, 1, 2, 1, 2, 1, 1, 1, 1, 1, 2, 1)
-    x = torch.from_numpy(np.random.Generator(np.random.PCG64(seed + 7919)).random((2, 3) + tuple(calib_hw)))
-    x = bn_act(F.conv2d(x, put('conv0.0.weight', gauss((enc[0], 3, 3, 3), 27)), None, 2, 1), enc[0], 'conv0.1', 6.0)
+    x = _probe(seed, calib_hw, in_channels)
+    x = bn_act(F.conv2d(x, put('conv0.0.weight', gauss((enc[0], in_channels, 3, 3), 9 * in_channels)), None, 2, 1), enc[0],
+               'conv0.1', 6.0)
     keep = {}
     for i in range(1, 14):
         ci, co = enc[i - 1], enc[i]
@@ -132,11 +144,26 @@ def synthetic_state_dict(widths=STOCK_WIDTHS, seed=1, calib_hw=(96, 128), skip='
     return {k: v.clone() for k, v in sd.items()}
 
 
-def synthetic_input(n, h, w, seed=0):
+SPARSE_DENSITY = 0.05          # fraction of pixels with a depth sample in a synthetic sparse-depth channel
+SPARSE_RANGE = (0.5, 10.0)     # metres, the NYU Depth v2 range
+
+
+def synthetic_input(n, h, w, seed=0, channels=3):
     """[n,3,h,w] fp32 in [0,1) -- the range the reference pipeline yields
-    (dataloaders/transforms.py:216-224, dataloaders/nyu.py:56)."""
+    (dataloaders/transforms.py:216-224, dataloaders/nyu.py:56).
+
+    ``channels != 3``: the input of a sparse-to-dense model, ``channels - 1`` image channels in [0, 1) and then one sparse
+    depth channel in metres: zero except at a ``SPARSE_DENSITY`` fraction of the pixels, where it is U(0.5, 10).  So 4 is
+    RGB-D and 1 is depth only.  ``channels=3`` is the draw above, unchanged."""
     rng = np.random.Generator(np.random.PCG64(seed))
-    return torch.from_numpy(rng.random((n, 3, h, w), dtype=np.float32))
+    if channels == 3:
+        return torch.from_numpy(rng.random((n, 3, h, w), dtype=np.float32))
+    if channels < 1:
+        raise ValueError('channels must be >= 1')
+    img = rng.random((n, channels - 1, h, w), dtype=np.float32)
+    hit = rng.random((n, 1, h, w)) < SPARSE_DENSITY
+    depth = np.where(hit, rng.uniform(SPARSE_RANGE[0], SPARSE_RANGE[1], (n, 1, h, w)), 0.0).astype(np.float32)
+    return torch.from_numpy(np.ascontiguousarray(np.concatenate([img, depth], axis=1)))
 
 
 def synthetic_target(pred, seed=1):
@@ -161,7 +188,7 @@ def to_mobilenet_keys(sd):
     return out
 
 
-def synthetic_nnconv_state_dict(kernel_size=5, seed=1, calib_hw=(96, 128)):
+def synthetic_nnconv_state_dict(kernel_size=5, seed=1, calib_hw=(96, 128), in_channels=3):
     """state_dict with the ``models.MobileNet('nnconv<k>')`` key schema (dense NNConv decoder, reference models.py:52-59,
     245-270): the encoder of ``synthetic_state_dict(STOCK_WIDTHS, seed)`` (renamed with ``to_mobilenet_keys``), then five
     dense ``conv(C, C/2, k)`` blocks and ``pointwise(32, 1)`` drawn from a separate seeded stream.
@@ -170,9 +197,10 @@ def synthetic_nnconv_state_dict(kernel_size=5, seed=1, calib_hw=(96, 128)):
     drawn as above and running statistics CALIBRATED in fp64 on the encoder output of the same probe batch, a positive head
     with gamma = 1, beta = 3.  Measured conditioning (storage-emulated forward against the fp32 forward, seed 1): fp16
     2.5e-3 at 2x64x96 but 1.5e-2 at 1x224x224 (bf16 2.5e-2 / 1.2e-1); calibrating the decoder on a 224 x 224 probe instead
-    does not change that.  The functions above are untouched, so their fixtures stay bit-identical."""
+    does not change that.  The functions above are untouched, so their fixtures stay bit-identical.  ``in_channels``: the
+    stem's input channels, as in ``synthetic_state_dict``."""
     import torch.nn.functional as F
-    base = to_mobilenet_keys(synthetic_state_dict(STOCK_WIDTHS, seed=seed, calib_hw=calib_hw))
+    base = to_mobilenet_keys(synthetic_state_dict(STOCK_WIDTHS, seed=seed, calib_hw=calib_hw, in_channels=in_channels))
     sd = {k: v for k, v in base.items() if k.startswith('mobilenet.')}
     f64 = torch.float64
 
@@ -184,7 +212,7 @@ def synthetic_nnconv_state_dict(kernel_size=5, seed=1, calib_hw=(96, 128)):
         return y.clamp(0.0, hi) if hi is not None else y.clamp_min(0.0)
 
     strides = (2, 1, 2, 1, 2, 1, 2, 1, 1, 1, 1, 1, 2, 1)
-    x = torch.from_numpy(np.random.Generator(np.random.PCG64(seed + 7919)).random((2, 3) + tuple(calib_hw)))
+    x = _probe(seed, calib_hw, in_channels)
     x = bn(F.conv2d(x, sd['mobilenet.0.0.weight'].to(f64), None, 2, 1), 'mobilenet.0.1', 6.0)
     for i in range(1, 14):
         ci = sd['mobilenet.%d.0.weight' % i].shape[0]
@@ -218,14 +246,15 @@ def synthetic_nnconv_state_dict(kernel_size=5, seed=1, calib_hw=(96, 128)):
     return sd
 
 
-def synthetic_convt_state_dict(decoder, seed=1, calib_hw=(96, 128)):
+def synthetic_convt_state_dict(decoder, seed=1, calib_hw=(96, 128), in_channels=3):
     """state_dict with the ``models.MobileNet(decoder)`` key schema for ``decoder`` in ``deconv3/5/7/9`` and ``upconv``
     (reference models.py:77-107, 145-201): the encoder of ``synthetic_state_dict(STOCK_WIDTHS, seed)`` (renamed with
     ``to_mobilenet_keys``), then five ``convt(C, C/2, k)`` (keys ``decoder.convt<j>.{0,1}.*``) or ``upconv(C, C/2)``
     blocks (``decoder.upconv<j>.{1,2}.*``) and ``convf = pointwise(32, 1)``, drawn from a separate seeded stream.
 
     The recipe of ``synthetic_nnconv_state_dict``: decoder weights U(-b, b) with b = 1/sqrt(k*k*C), BN gamma / beta drawn
-    as there, running statistics CALIBRATED in fp64 on the same probe batch, a positive head with gamma = 1, beta = 3."""
+    as there, running statistics CALIBRATED in fp64 on the same probe batch, a positive head with gamma = 1, beta = 3.
+    ``in_channels``: the stem's input channels, as in ``synthetic_state_dict``."""
     import torch.nn.functional as F
     if decoder == 'upconv':
         k, child, conv_i, bn_i = 5, 'upconv', 1, 2
@@ -233,7 +262,7 @@ def synthetic_convt_state_dict(decoder, seed=1, calib_hw=(96, 128)):
         k, child, conv_i, bn_i = int(decoder[6]), 'convt', 0, 1
     else:
         raise ValueError('no synthetic recipe for decoder %r' % decoder)
-    base = to_mobilenet_keys(synthetic_state_dict(STOCK_WIDTHS, seed=seed, calib_hw=calib_hw))
+    base = to_mobilenet_keys(synthetic_state_dict(STOCK_WIDTHS, seed=seed, calib_hw=calib_hw, in_channels=in_channels))
     sd = {key: v for key, v in base.items() if key.startswith('mobilenet.')}
     f64 = torch.float64
 
@@ -245,7 +274,7 @@ def synthetic_convt_state_dict(decoder, seed=1, calib_hw=(96, 128)):
         return y.clamp(0.0, hi) if hi is not None else y.clamp_min(0.0)
 
     strides = (2, 1, 2, 1, 2, 1, 2, 1, 1, 1, 1, 1, 2, 1)
-    x = torch.from_numpy(np.random.Generator(np.random.PCG64(seed + 7919)).random((2, 3) + tuple(calib_hw)))
+    x = _probe(seed, calib_hw, in_channels)
     x = bn(F.conv2d(x, sd['mobilenet.0.0.weight'].to(f64), None, 2, 1), 'mobilenet.0.1', 6.0)
     for i in range(1, 14):
         ci = sd['mobilenet.%d.0.weight' % i].shape[0]

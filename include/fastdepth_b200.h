@@ -74,7 +74,7 @@ typedef enum { FD_ACT_RELU = 0, FD_ACT_RELU6 = 1 } fd_act;
 
 typedef struct {
     int32_t kind;        /* fd_stage_kind                                                    */
-    int32_t c_in;        /* input channels  (3 for the stem)                                 */
+    int32_t c_in;        /* input channels; the stem's is x's: 1..7 (3 RGB, 1 depth, 4 RGB-D) */
     int32_t c_out;       /* output channels (1 for the head)                                 */
     int32_t ksize;       /* spatial kernel: 3 (stem, encoder dw), 5 (decoder dw), 1 (head)   */
     int32_t stride;      /* stride of the spatial conv (1 or 2)                              */
@@ -90,7 +90,9 @@ typedef struct {
 /* Build a plan for a stage list (always: 1 STEM, k stages each DWPW, CONV, DECONV or UPCONV, 1 HEAD) at a fixed problem size.
  * Allocates NHWC activation buffers and packed-weight storage on `device`.
  * H and W must be multiples of 32 (reference forward's skip shapes only line up then),
- * every c_in/c_out except the stem's c_in and the head's c_out a multiple of 8. */
+ * every c_in/c_out except the stem's c_in and the head's c_out a multiple of 8.  The stem's c_in is the channel count of x:
+ * 1..7 (x is [N,c_in,H,W]; K = 9 c_in fits one 64-element K row of the tensor-core stem).  c_in <= 0 fails with
+ * FD_ERR_INVALID, c_in >= 8 with FD_ERR_UNSUPPORTED. */
 int fd_plan_create(const fd_stage_desc* stages, int n_stages,
                    int n, int h, int w, int dtype /* fd_dtype */, int device, fd_plan** out);
 
@@ -159,7 +161,7 @@ int fd_plan_set_stage_weights(fd_plan* plan, int stage,
 int fd_plan_set_option(fd_plan* plan, const char* name, int value);
 int fd_plan_get_option(fd_plan* plan, const char* name, int* value);
 
-/* The hot path.  x_dev: [N,3,H,W] contiguous, plan dtype.  y_dev: [N,1,H,W] contiguous,
+/* The hot path.  x_dev: [N,c_in,H,W] contiguous, plan dtype, c_in the stem's.  y_dev: [N,1,H,W] contiguous,
  * plan dtype.  Enqueues on `stream`; returns without synchronising.  A plan owns one set of activation
  * buffers: calls on different streams are ordered after each other by an event (never corrupted, never
  * overlapped); to keep several forwards in flight use several plans (one per stream).
@@ -167,19 +169,19 @@ int fd_plan_get_option(fd_plan* plan, const char* name, int* value);
 int fd_forward(fd_plan* plan, const void* x_dev, void* y_dev, void* stream);
 
 /* The same forward over the first n images, 1 <= n <= the plan's N, at the plan's own H x W: fd_forward_shape(plan, n, H,
- * W, ...).  x_dev is [n,3,H,W] and y_dev [n,1,H,W]. */
+ * W, ...).  x_dev is [n,c_in,H,W] and y_dev [n,1,H,W]. */
 int fd_forward_batch(fd_plan* plan, int n, const void* x_dev, void* y_dev, void* stream);
 
-/* The forward of n images at any resolution h x w that fits the plan's pixel capacity: x_dev is [n,3,h,w] and y_dev
+/* The forward of n images at any resolution h x w that fits the plan's pixel capacity: x_dev is [n,c_in,h,w] (c_in the stem's) and y_dev
  * [n,1,h,w], contiguous, plan dtype.  Accepted: n >= 1, h and w positive multiples of 32, n*h*w <= N*H*W (every stage
  * buffer of the plan is dense NHWC of N*(H/s)*(W/s)*C elements, so the request fits in its front).  Anything else fails
  * with FD_ERR_INVALID; for a request that does not fit, the message names the capacity in pixels and the plan's (N, H, W).
- * Nothing is read or written past n*h*w elements of x_dev (times 3) or y_dev.  The result equals that of a plan built for
+ * Nothing is read or written past n*h*w elements of x_dev (times c_in) or y_dev.  The result equals that of a plan built for
  * (n, h, w), bit for bit.  The plan builds the steps for (n, h, w) on first use (every stage's geometry, planner choices,
  * grids, tensor maps, whether a run of blocks takes the chain kernel) over its own activation buffers, packed weights and
  * split weights; it keeps up to 8 such step sets, least recently used first out (the set of its own (N, H, W) is always
  * kept), and captures graphs per (x_dev, y_dev, n, h, w).  fd_forward(plan, ...) is fd_forward_shape(plan, N, H, W, ...).
- * fd_forward_host and fd_pipeline_* always run N images at H x W. */
+ * fd_forward_host and fd_pipeline_* always run N images at H x W, and copy N*c_in*H*W elements of x. */
 int fd_forward_shape(fd_plan* plan, int n, int h, int w, const void* x_dev, void* y_dev, void* stream);
 
 /* Same, end to end from HOST buffers: H2D copy of x, forward, D2H copy of y, then waits for
@@ -264,7 +266,9 @@ int fd_debug_pw_plan(int h_out, int w_out, int n, int c_in, int c_out, int upsam
 /* Debug (host only, needs no GPU): whether a 16-bit plan on path 1 of these stages at n x h x w runs its stem and the two
  * blocks after it as one front_tc_kernel step ("front"), and that kernel's budget.  out[0] = 1 when it does, out[1] = its
  * items (8x8 tiles of conv2's map, 0 when it does not), out[2] = dynamic shared memory per CTA in bytes, out[3] = CTAs per
- * SM, out[4] = threads per CTA, out[5..7] = bytes of its weight + parameter, A-operand and tile regions.  cap >= 8. */
+ * SM, out[4] = threads per CTA, out[5..7] = bytes of its weight + parameter, A-operand and tile regions.  The budget is the
+ * one for the stem's c_in: the x box holds c_in planes, c_in <= 3 fit inside the A region, c_in = 4 grows it by 2688 bytes
+ * and c_in >= 5 would leave one CTA per SM, so the route is taken for c_in 1..4 only.  cap >= 8. */
 int fd_debug_front_plan(const fd_stage_desc* stages, int n_stages, int dtype, int n, int h, int w, int* out, int cap);
 
 int fd_debug_convt_plan(int kind, int ksize, int h_in, int w_in, int n, int c_in, int c_out, int n_sms, int* out, int cap);

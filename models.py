@@ -275,8 +275,13 @@ class MobileNet(nn.Module):
         per term, each within 3*2^-22 of the exact product), which keeps the result within the fp32 bound of 1e-3.  Under
         the default ``'highest'`` it stays on stock PyTorch.  The rule is the fp32 accuracy contract, not speed: stock
         PyTorch runs these convs under cuDNN's default TF32 conv precision, about 1e-2 away on the NNConv5 golden, and
-        split TF32 is within the bound; a user who asks for ``'high'`` gets the faster, still fp32-accurate path."""
-        fused_ok = (x.is_cuda and not self.training and x.dim() == 4 and x.shape[1] == 3 and
+        split TF32 is within the bound; a user who asks for ``'high'`` gets the faster, still fp32-accurate path.
+
+        ``in_channels`` from 1 to 7 (depth only: 1, RGB-D: 4) routes the same way when ``x`` has that many channels; the
+        engine's stem reads them all.  8 or more channels, or an input whose channel count differs from the stem's, stays
+        on stock PyTorch (which raises for the latter)."""
+        c_in = self.mobilenet[0][0].weight.shape[1]
+        fused_ok = (x.is_cuda and not self.training and x.dim() == 4 and x.shape[1] == c_in and 1 <= c_in <= 7 and
                     x.shape[2] % 32 == 0 and x.shape[3] % 32 == 0)     # what the fused plan covers; anything else: stock PyTorch
         if fused_ok:
             from fastdepth_b200 import plan as _plan
